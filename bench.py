@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — MCTS simulations/s of the B200 self-play hot path (BASELINE.json metric).
+"""bench.py — MCTS simulations/s of the H100 self-play hot path (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            our arm (one process per GPU under torchrun for N > 1)
   python bench.py --impl reference ...                      CPU arm: the reference's OWN `run.py self` plumbing on host cores
@@ -33,14 +33,6 @@ WORKLOADS = {
 }
 CONFIG_INDEX = dict(c2=1, c3=2, c5=4)
 
-# DRAM bytes (dram__bytes_read.sum + dram__bytes_write.sum) per launch of the dominant kernel from `ncu --set full` (None where no
-# capture exists).  c3, 8192-board launches (profiles/r02i_conv_256_ncu_raw_subset.csv): conv1 (k_igemm3, fp16 in / out)
-# 0.332 + 0.290 GB, conv2 (k_igemm2, + fp32 skip in / fp32 copy out) 1.399 + 0.943 GB; mean of the two = one launch of the
-# tower on average.  Algorithmic bytes: 0.754 GB and 2.264 GB (conv1 reads part of its input from L2: 126 MB of the 377 MB
-# the previous launch wrote).  c2, 2048-board launches (r02i_conv_128_*): 0.057 / 0.118 GB (activations are L2-resident).
-NCU_TRAFFIC = {("c3", 1024, 8): 1.482e9, ("c2", 256, 8): 0.0875e9}
-
-
 def net_flops(filters, blocks):
     return 2 * 90 * (350 * filters + blocks * 18 * filters * filters + 6 * filters) + 2 * (360 * 2086 + 180 * 256 + 256)
 
@@ -51,12 +43,9 @@ def workload_text(name, games, sims, filters, blocks):
 
 
 def measured_peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
-            d = json.load(f)
-        return float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1428.0))), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
-    return 1400.0, "fallback (B200_PROFILING.md sustained ~1.4 PFLOP/s)"
+    """Dense FP16 tensor peak the conv tower is compared against: NVIDIA's H100 SXM data sheet figure (700 W card).  It is a
+    ceiling, not a rate this code has reached; a card with a lower power limit (see `clocks`) sustains less."""
+    return 989.0, "NVIDIA H100 SXM data sheet, dense FP16 (not measured)"
 
 
 class ClockSampler:
@@ -232,14 +221,8 @@ def run_reference_arm(args):
 
 
 def conv_kernel_names(filters):
-    """The residual-conv kernels cz_nn.cu's launch selection runs at this width (use_tma_epilogue_for): all-TMA-epilogue pair kernel,
-    two M-tiles per CTA at C <= 128; the fp32-skip conv2 of the 256-wide tower keeps the round-1 pair kernel."""
-    if filters <= 128:
-        return f"igemm::k_igemm3<{filters}, 2> (3x3 residual conv, tcgen05 cta_group::2, two M-tiles per CTA)"
-    if filters >= 256:
-        return (f"igemm::k_igemm3<{filters}, 1> (conv1) + igemm::k_igemm2<{filters}> (conv2, fp32 skip stream): 3x3 residual conv, "
-                "tcgen05 cta_group::2")
-    return f"igemm::k_igemm3<{filters}, 1> (3x3 residual conv, tcgen05 cta_group::2)"
+    """The residual-conv kernel cz_nn.cu launches at this width for the full-size batches of the benchmark."""
+    return f"igemm::k_igemm<{filters}> (3x3 residual conv, implicit GEMM on wgmma, im2col TMA)"
 
 
 def bench_config(workload, games, sims, filters, blocks, K, world=1, skip_stream="auto"):
@@ -249,9 +232,9 @@ def bench_config(workload, games, sims, filters, blocks, K, world=1, skip_stream
     return {"workload": workload_text(workload, games, sims, filters, blocks), "games_per_gpu": games, "sims_per_move": sims,
             "leaves_per_round": K, "net": f"{filters}x{blocks}", "skip_stream": skip_stream,
             "parallelism": f"dp{world} (games sharded, no data-path collective; finished-game rings all_gathered every step)",
-            "l2": (f"GPU arm: activations {act_mb:.0f} MB per round + tree pools stream through HBM (> 126 MB L2, no flush needed)"
-                   if act_mb > 2 * 126 else
-                   f"GPU arm: activations {act_mb:.0f} MB per round fit the 126 MB L2 and are NOT flushed between steps (secondary "
+            "l2": (f"GPU arm: activations {act_mb:.0f} MB per round + tree pools stream through HBM (> 50 MB L2, no flush needed)"
+                   if act_mb > 2 * 50 else
+                   f"GPU arm: activations {act_mb:.0f} MB per round fit the 50 MB L2 and are NOT flushed between steps (secondary "
                    f"workload; the headline workload c3 streams 1.1 GB per round)")}
 
 
@@ -344,6 +327,8 @@ def measure(args, workload, steps, warmup, world, rank, local, dist, want_e2e=Tr
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and workload == args.workload and rank == 0:
+        dump_outputs(eng, args.dump_outputs)
     launches = eng.launch_count() - launches0
     st1, c1 = eng.search_stats(), eng.counters()
     gather_ms = sum(a.elapsed_time(b) for a, b in gather_ev)
@@ -407,7 +392,6 @@ def measure(args, workload, steps, warmup, world, rank, local, dist, want_e2e=Tr
             "nn_positions_per_sec": (st1["nodes_created"] - st0["nodes_created"]) * world / (ms * 1e-3),
             "gpu_launches": int(launches),
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                         "traffic": NCU_TRAFFIC.get((workload, games, K)),
                          "kernel": conv_kernel_names(filters),
                          "launches": int(conv_launches), "avg_launch_ms": conv_ms / max(1.0, conv_launches / world),
                          "peak_source": peak_src, "share_of_step": conv_ms / ms_prof,
@@ -440,6 +424,23 @@ def measure(args, workload, steps, warmup, world, rank, local, dist, want_e2e=Tr
     return out
 
 
+def dump_outputs(eng, out_dir):
+    """What the last timed step handed back to its caller, as float32 .npy files: every game's position after the move
+    (packed board bytes), the legal moves at that position, their visit counts (the subtree the search keeps) and the
+    simulations each game ran.  With the same arguments the games start from the same seeded state, so two builds can be
+    compared output for output."""
+    import numpy as np
+    from cczero_b200 import records as rec
+    os.makedirs(out_dir, exist_ok=True)
+    stage = rec.RootStage(eng)
+    boards = eng.download_roots(stage).numpy()
+    n, moves, counts = (t.numpy() for t in eng.download_root_stats(stage))
+    arrays = {"root_boards": boards, "root_moves": moves, "root_visits": n, "root_move_counts": counts,
+              "root_sims_run": stage.sims.numpy()}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
+
+
 FUSED_POLICY = True      # flipped when the integrated search gathers legal logits itself (no [B][2086] f32 policy row)
 
 
@@ -451,15 +452,13 @@ def policy_bytes_per_leaf(legal):
 
 def uci_latency_block():
     """Single-game latency path (SURVEY §8f rank 4): `go depth 8` (800 simulations, search_threads 10) through the drop-in
-    `CChessPlayer(uci=True)` on the reference's trained 192x10 weights (committed fixture), wall clock around `action()`, with the
+    `CChessPlayer(uci=True)` on seeded random-init 192x10 weights, wall clock around `action()`, with the
     nps figure the REFERENCE's formula gives (agent/player.py:446-447).  tools/bench_uci.py is the measurement."""
     try:
         import importlib.util
         spec = importlib.util.spec_from_file_location("bench_uci", os.path.join(ROOT, "tools", "bench_uci.py"))
         mod = importlib.util.module_from_spec(spec)
         spec.loader.exec_module(mod)
-        if not os.path.exists(os.path.join(ROOT, "tests", "golden", "model_best_192x10.npz")):
-            return {"error": "tests/golden/model_best_192x10.npz missing"}
         weights, src = mod.load_weights(192, 10)
         keep = os.environ.get("CZ_SEARCH_LOOP")
         try:
@@ -538,6 +537,8 @@ def main():
                     "values make games finish inside a short run so that the record gather / file writes carry data")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the short c2 / c5 runs (and the c1 / free-NN legs of the CPU arm)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed for its caller as DIR/<name>.npy (float32)")
     ap.add_argument("--skip-stream", default="auto", choices=["auto", "fp32", "fp16"],
                     help="precision of the residual skip stream (auto = fp32 beyond 10 blocks: keeps the 1e-3 parity bound)")
     args = ap.parse_args()

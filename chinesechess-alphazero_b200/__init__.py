@@ -1,4 +1,4 @@
-"""cczero-b200: B200-native Xiangqi self-play hot path behind the reference's
+"""cczero-b200: H100-native Xiangqi self-play hot path behind the reference's
 CChessPlayer / CChessModelAPI / SelfPlayWorker surface.
 
 The directory name carries the reference's name and is not a Python identifier; import it as

@@ -1,6 +1,6 @@
 """`CChessModelAPI` drop-in (reference: cchess_alphazero/agent/api.py:16-117): the batching prediction server.
 
-Same wire protocol as the reference, so UNMODIFIED reference players can be served by the B200 network:
+Same wire protocol as the reference, so UNMODIFIED reference players can be served by the GPU network:
 a client sends `list[np.float32[14,10,9]]` (`[28,10,9]` for a use_history network) on its pipe end, the server answers `list[(np.float32[2086], float)]`
 in the same order (api.py:48-74 <-> player.py:118-120,131-140).  One daemon thread waits on every pipe, drains
 what is ready, runs ONE batched forward (`cz_nn_forward`: tensor-core pipeline) and scatters the results.

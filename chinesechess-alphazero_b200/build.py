@@ -1,10 +1,10 @@
 """Build recipe for the native code of cczero-b200.
 
-`build_cuda()`  -> chinesechess-alphazero_b200/libcczero_b200.so   (nvcc, sm_100a; THE product)
+`build_cuda()`  -> chinesechess-alphazero_b200/libcczero_b200.so   (nvcc, sm_90a; THE product)
 `build_emul()`  -> tests/simt_emul/libcz_emul.so                   (g++ -DCZ_EMUL; test tier only)
 
 Both are built in-tree so the .so travels with the repo snapshot to the GPU box.
-nvcc cross-compiles sm_100a without a GPU.
+nvcc cross-compiles sm_90a without a GPU.
 """
 import hashlib
 import os
@@ -25,7 +25,7 @@ INT_UNITS = ["cz_env_api.cu", "cz_tree_api.cu"]
 NN_UNITS = ["cz_nn.cu"]
 HOST_UNITS = ["cz_err.cpp"]
 
-NVCC_COMMON = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_COMMON = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
                "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include")]
 
 

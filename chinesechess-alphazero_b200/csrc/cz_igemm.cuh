@@ -1,45 +1,51 @@
 // cz_igemm.cuh — the one dense contraction of the hot path: implicit-GEMM 3x3 convolution (and the
-// plain GEMM of the policy head) on tcgen05 tensor cores, TMEM accumulators, TMA-fed operands.
+// plain GEMM of the policy head) on Hopper warpgroup tensor cores (wgmma), TMA-fed operands.
 //
 // Replaces the Conv2D/BatchNormalization/Add/Activation stack of agent/model.py:68-83 (residual
 // block) and the Dense of :54 (policy_out) that the reference runs through Keras/TF/cuDNN.
 //
-// Activation layout in HBM ("strip" layout): fp16 [n_boards*11][9][C].  Board b occupies strip rows
-//   b*11 .. b*11+9 (network row r = 9 - y), strip row b*11+10 is an all-zero separator shared as the
-//   vertical halo of board b (below) and b+1 (above).  Horizontal halo and the rows above board 0 /
-//   below the last board come from TMA out-of-bounds zero fill.  A 3x3 tap (dy,dx) is therefore ONE
-//   TMA box load at coordinates (c0, dx, r0+dy): no im2col, no masking in the MMA.
-// Tile: 14 strip rows x 9 columns = 126 pixels -> UMMA M = 128 (rows 126,127 are don't-care: an A row
-//   only feeds the same D row), N = N_TILE output channels (<= 256), K walks taps x C_in in 64-channel
-//   blocks (128-byte swizzled rows).  Useful fraction of the MMA work: (90/99)*(126/128) = 89.5 %.
-// Pipeline: warp 0 = TMA producer, warp 1 = MMA issuer (one thread), warp 2 = TMEM allocator,
-//   warps 4-7 = epilogue (TMEM -> registers -> +bias (+residual) -> ReLU -> fp16 -> HBM).  kStages-deep
-//   smem ring (full/empty mbarriers) and two TMEM accumulators (tfull/tempty) so the epilogue of tile i
-//   overlaps the MMAs of tile i+1.  Persistent: grid = #SMs, tiles strided over CTAs.
+// Activation layouts in HBM (fp16, channels contiguous):
+//   dense  (conv == 2, the production layout): [n_boards*90][C] pixels.  A 3x3 tap (dy,dx) of 128 consecutive output pixels
+//          is ONE im2col-mode TMA load (64 channels x 128 pixels); taps outside the board are zero-filled by the TMA unit and
+//          the 128-pixel column walks across rows and boards.
+//   strip  (conv == 1): [n_boards*11][9][C].  Board b occupies strip rows b*11 .. b*11+9 (network row r = 9 - y), strip row
+//          b*11+10 is an all-zero separator shared as the vertical halo of board b (below) and b+1 (above).  A tap is ONE
+//          tiled TMA box load at coordinates (c0, dx, r0+dy) of 14 strip rows x 9 columns = 126 pixels (rows 126,127 of the
+//          M tile are don't-care: an A row only feeds the same D row).
+//   GEMM   (conv == 0): A [M][K] rows, 128 per tile.
+// Tile: M = 128 pixels / rows, N = N_TILE output channels (<= 256), K walks taps x C_in in 64-channel blocks (128-byte
+//   swizzled rows).  Every output element accumulates its K blocks in the same order whatever the tile shape, so results do
+//   not depend on N_TILE or on how the M tiles are spread over CTAs.
+// CTA = 3 warpgroups: warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers, each issuing m64nN wgmma
+//   on its 64 rows of the tile with fp32 accumulators in registers, then running the epilogue from those registers
+//   (+bias (+residual) -> ReLU -> fp16 / fp32 -> HBM).  kStages-deep smem ring with full/empty mbarriers; the producer runs
+//   ahead into the next tile while the consumers store the current one.  Persistent: grid <= #SMs, tiles strided over CTAs.
 #pragma once
 #include <cuda_fp16.h>
-#include "cz_umma.cuh"
+#include "cz_wgmma.cuh"
 
 namespace igemm {
 
-constexpr int kStages = 4;
 constexpr int kBlockK = 64;                 // fp16 per k-block row = 128 B = swizzle span
 constexpr int kTileM = 128;
 constexpr int kAStageBytes = kTileM * 128;  // 16 KB
-constexpr int kThreads = 256;
+constexpr int kThreads = 384;
+constexpr int kConsumerWarps = 8;
+constexpr int kSmemLimit = 232448;          // opt-in dynamic shared memory per CTA on sm_90 (227 KB)
+constexpr int kMaxStages = 8;
 
 struct Args {
   int n_taps;        // 9 (3x3 conv) or 1 (plain GEMM)
   int k_chunks;      // C_in / 64
-  int m_tiles;       // ceil(rows / box_r)
+  int m_tiles;       // ceil(rows / pixels per tile) (an upper bound when n_dev is set)
   int n_tiles;       // ceil(N / N_TILE)
-  int box_w;         // 9 (conv) or 1 (GEMM)
-  int box_r;         // 14 (conv) or 128 (GEMM): A-box extent along the outer row dimension
-  int rows;          // conv: strip rows (n_boards*11); GEMM: M
+  int box_w;         // 9 (strip conv) or 1 (GEMM)
+  int box_r;         // 14 (strip conv) or 128 (GEMM): A-box extent along the outer row dimension
+  int rows;          // strip conv: strip rows (n_boards*11); dense conv: pixels; GEMM: M
   int n_total;       // B-operand rows per tap (C_out padded to N_TILE multiple)
   int n_valid;       // real number of output columns
   int ldo;           // output leading dimension in elements
-  int conv;          // 1: strip layout, separator rows forced to zero; 2: dense [B*90][C] pixels fed by im2col TMA
+  int conv;          // 1: strip layout, separator rows forced to zero; 2: dense [B*90][C] pixels fed by im2col TMA; 0: GEMM
   int relu;
   int out_f32;       // 1: float output (GEMM logits), 0: fp16
   const float* bias; // [n_total] or null
@@ -64,108 +70,109 @@ template <int N_TILE>
 struct Cfg {
   static constexpr int kBStageBytes = N_TILE * 128;
   static constexpr int kStageBytes = kAStageBytes + kBStageBytes;
-  static constexpr int kTmemCols = (2 * N_TILE <= 32) ? 32 : (2 * N_TILE <= 64) ? 64 : (2 * N_TILE <= 128) ? 128
-                                   : (2 * N_TILE <= 256) ? 256 : 512;
-  static constexpr int kSmemBytes = kStages * kStageBytes + 256 + 1024;  // + barriers + alignment slack
-  static_assert(2 * N_TILE <= 512, "two accumulators must fit TMEM");
-  static_assert(N_TILE % 16 == 0 && N_TILE >= 16 && N_TILE <= 256, "UMMA N constraint for M=128");
+  static constexpr int kFit = (kSmemLimit - 256 - 1024) / kStageBytes;
+  static constexpr int kStages = kFit > kMaxStages ? kMaxStages : kFit;   // 4 (N = 256) .. 8 (N = 64)
+  static constexpr int kSmemBytes = kStages * kStageBytes + 256 + 1024;    // + barriers + alignment slack
+  static_assert(N_TILE % 64 == 0 && N_TILE <= 256, "wgmma N tile");
 };
 
 template <int N_TILE>
 __global__ void __launch_bounds__(kThreads, 1)
 k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Args a) {
   using C = Cfg<N_TILE>;
+  constexpr int S = C::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * C::kStageBytes);
-  uint64_t* full = bars;                 // [kStages]  TMA -> MMA
-  uint64_t* empty = bars + kStages;      // [kStages]  MMA -> TMA
-  uint64_t* tfull = bars + 2 * kStages;  // [2]        MMA -> epilogue
-  uint64_t* tempty = tfull + 2;          // [2]        epilogue -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * C::kStageBytes);   // [S]  TMA -> MMA
+  uint64_t* empty = full + S;                                                 // [S]  MMA -> TMA (one arrive per consumer warp)
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
-    umma::prefetch_tmap(&tmA);
-    umma::prefetch_tmap(&tmB);
+  const int wgi = threadIdx.x >> 7, t = threadIdx.x & 127;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < S; ++s) { wg::mbar_init(&full[s], 1); wg::mbar_init(&empty[s], kConsumerWarps); }
+    wg::fence_barrier_init();
   }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStages; ++s) { umma::mbar_init(&full[s], 1); umma::mbar_init(&empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { umma::mbar_init(&tfull[i], 1); umma::mbar_init(&tempty[i], 128); }
-    umma::fence_barrier_init();
-    umma::fence_proxy_async();
-  }
-  if (warp == 2) umma::tmem_alloc<C::kTmemCols>(tmem_slot);
-  umma::tc_fence_before();
+  wg::griddep_launch_dependents();     // (PDL launches only) the next conv may become resident while this one runs
   __syncthreads();
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  wg::griddep_wait();                  // (PDL launches only) the producer of this conv's input has completed
 
   const int n_kb = a.n_taps * a.k_chunks;
   const int rows = args_rows(a);
-  const int m_tiles = a.n_dev ? (rows + a.box_r * a.box_w - 1) / (a.box_r * a.box_w) : a.m_tiles;   // n_dev: GEMM / dense modes only
+  const int m_tiles = a.conv == 1 ? a.m_tiles : (rows + kTileM - 1) / kTileM;
   const int total_tiles = m_tiles * a.n_tiles;
 
-  if (warp == 0) {
+  if (wgi == 0) {
     // ------------------------------------------------------------ TMA producer
-    if (lane == 0) {
-      uint32_t it = 0;
+    if (t == 0) {
+      wg::prefetch_tmap(&tmA);
+      wg::prefetch_tmap(&tmB);
+      uint32_t s = 0, ph = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int m_tile = tile % m_tiles, n_tile = tile / m_tiles;
+        // dense mode: first output pixel of this tile as (image, row, column); im2col walks on from there
+        const int pix0 = m_tile * kTileM, img0 = pix0 / 90, row0 = (pix0 % 90) / 9, col0 = pix0 % 9;
         for (int tap = 0; tap < a.n_taps; ++tap) {
           const int dy = a.n_taps == 9 ? tap / 3 - 1 : 0;
           const int dx = a.n_taps == 9 ? tap % 3 - 1 : 0;
-          for (int kc = 0; kc < a.k_chunks; ++kc, ++it) {
-            const uint32_t s = it % kStages, ph = (it / kStages) & 1;
-            umma::mbar_wait(&empty[s], ph ^ 1);
+          for (int kc = 0; kc < a.k_chunks; ++kc) {
+            wg::mbar_wait(&empty[s], ph ^ 1);
             uint8_t* sA = smem + s * C::kStageBytes;
             uint8_t* sB = sA + kAStageBytes;
-            umma::mbar_expect_tx(&full[s], a.a_bytes + (uint32_t)C::kBStageBytes);
-            umma::tma_load_3d(sA, &tmA, &full[s], kc * kBlockK, dx, m_tile * a.box_r + dy);
-            umma::tma_load_2d(sB, &tmB, &full[s], kc * kBlockK, tap * a.n_total + n_tile * N_TILE);
+            wg::mbar_expect_tx(&full[s], a.a_bytes + (uint32_t)C::kBStageBytes);
+            if (a.conv == 2)
+              wg::tma_load_im2col_4d(sA, &tmA, &full[s], kc * kBlockK, col0 - 1, row0 - 1, img0, (uint16_t)(dx + 1), (uint16_t)(dy + 1));
+            else
+              wg::tma_load_3d(sA, &tmA, &full[s], kc * kBlockK, dx, m_tile * a.box_r + dy);
+            wg::tma_load_2d(sB, &tmB, &full[s], kc * kBlockK, tap * a.n_total + n_tile * N_TILE);
+            if (++s == (uint32_t)S) { s = 0; ph ^= 1; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma::idesc_f16(kTileM, N_TILE);
-      uint32_t it = 0, tcount = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tcount) {
-        const uint32_t acc = tcount & 1, aph = (tcount >> 1) & 1;
-        umma::mbar_wait(&tempty[acc], aph ^ 1);
-        umma::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * N_TILE;
-        for (int kb = 0; kb < n_kb; ++kb, ++it) {
-          const uint32_t s = it % kStages, ph = (it / kStages) & 1;
-          umma::mbar_wait(&full[s], ph);
-          umma::tc_fence_after();
-          const uint32_t sA = umma::smem_u32(smem + s * C::kStageBytes);
-          const uint64_t da = umma::smem_desc_sw128(sA);
-          const uint64_t db = umma::smem_desc_sw128(sA + kAStageBytes);
+    return;
+  }
+
+  // -------------------------------------------------------------- consumers: MMA + epilogue on rows cw*64 .. cw*64+63
+  const int cw = wgi - 1, warp = t >> 5, lane = t & 31;
+  const int mrow = cw * 64 + warp * 16 + (lane >> 2);       // accumulator rows mrow and mrow + 8 of the tile
+  const int cq = 2 * (lane & 3);                            // first of the two adjacent columns per 8-column group
+  float acc[N_TILE / 2];
+  uint32_t s = 0, ph = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    const int m_tile = tile % m_tiles, n_tile = tile / m_tiles;
+    uint32_t prev = 0;
+    for (int kb = 0; kb < n_kb; ++kb) {
+      wg::mbar_wait(&full[s], ph);
+      const uint32_t sA = wg::smem_u32(smem + s * C::kStageBytes);
+      const uint64_t da = wg::smem_desc_sw128(sA + cw * 64 * 128);
+      const uint64_t db = wg::smem_desc_sw128(sA + kAStageBytes);
+      wg::wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k)   // +32 B per UMMA_K step inside the swizzle atom
-            umma::mma_f16_ss(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-          umma::mma_commit(&empty[s]);
-        }
-        umma::mma_commit(&tfull[acc]);
+      for (int k = 0; k < kBlockK / 16; ++k)                // +32 B per k16 step inside the swizzle atom
+        wg::Wgmma<N_TILE>::mma(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) != 0);
+      wg::wgmma_commit();
+      wg::wgmma_wait<1>();                                  // the previous stage's MMAs are done: hand it back to the producer
+      if (kb > 0 && lane == 0) wg::mbar_arrive(&empty[prev]);
+      prev = s;
+      if (++s == (uint32_t)S) { s = 0; ph ^= 1; }
+    }
+    wg::wgmma_wait<0>();
+    if (lane == 0) wg::mbar_arrive(&empty[prev]);
+
+    // ------------------------------------------------------------ epilogue
+    const int nb = n_tile * N_TILE + cq;                    // column of acc[4j + 2h] is nb + 8j
+    if (a.bias) {
+#pragma unroll
+      for (int j = 0; j < N_TILE / 8; ++j) {                // bias arrays are padded to the N tile
+        const float2 b = __ldg(reinterpret_cast<const float2*>(a.bias + nb + 8 * j));
+        acc[4 * j] += b.x; acc[4 * j + 1] += b.y; acc[4 * j + 2] += b.x; acc[4 * j + 3] += b.y;
       }
     }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------ epilogue
-    const int q = warp - 4;                 // TMEM lane quarter this warp may read
-    const int m = q * 32 + lane;            // accumulator row == pixel inside the tile
-    uint32_t tcount = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++tcount) {
-      const int m_tile = tile % m_tiles, n_tile = tile / m_tiles;
-      const uint32_t acc = tcount & 1, aph = (tcount >> 1) & 1;
-      umma::mbar_wait(&tfull[acc], aph);
-      umma::tc_fence_after();
-      long long grow;       // global output row
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = mrow + 8 * h;                           // accumulator row == pixel / row inside the tile
+      long long grow;                                       // global output row
       bool valid, zero = false;
-      if (a.conv) {
+      if (a.conv == 1) {
         const int srow = m_tile * a.box_r + m / 9;          // strip row
         valid = m < a.box_r * 9 && srow < rows;
         zero = (srow % 11) == 10;                           // separator row stays zero
@@ -174,343 +181,55 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
         grow = (long long)m_tile * kTileM + m;
         valid = grow < rows;
       }
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + acc * N_TILE;
-      float row_max = -INFINITY, row_sum = 0.f;
-      if (a.row_stats) {                                    // pass 1 over the accumulator: the row maximum of this N tile
-#pragma unroll 1
-        for (int c0 = 0; c0 < N_TILE; c0 += 32) {
-          uint32_t v[32];
-          umma::tmem_ld_32x32(t_row + c0, v);
-          const int n0 = n_tile * N_TILE + c0;
+      if (a.out_f32) {
+        if (a.row_stats) {                                  // the 4 threads of a quad hold one row: reduce across them
+          float mx = -INFINITY;
 #pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (n0 + j < a.n_valid) row_max = fmaxf(row_max, __uint_as_float(v[j]) + (a.bias ? __ldg(a.bias + n0 + j) : 0.f));
+          for (int j = 0; j < N_TILE / 8; ++j) {
+            if (nb + 8 * j < a.n_valid) mx = fmaxf(mx, acc[4 * j + 2 * h]);
+            if (nb + 8 * j + 1 < a.n_valid) mx = fmaxf(mx, acc[4 * j + 2 * h + 1]);
+          }
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          float sum = 0.f;
+#pragma unroll
+          for (int j = 0; j < N_TILE / 8; ++j) {
+            if (nb + 8 * j < a.n_valid) sum += __expf(acc[4 * j + 2 * h] - mx);
+            if (nb + 8 * j + 1 < a.n_valid) sum += __expf(acc[4 * j + 2 * h + 1] - mx);
+          }
+          sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+          sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+          if (valid && (lane & 3) == 0) a.row_stats[grow * a.n_tiles + n_tile] = make_float2(mx, sum);
         }
-      }
-#pragma unroll 1
-      for (int c0 = 0; c0 < N_TILE; c0 += 32) {
-        uint32_t v[32];
-        umma::tmem_ld_32x32(t_row + c0, v);
-        const int n0 = n_tile * N_TILE + c0;
-        if (valid && n0 < a.n_valid) {
-          float f[32];
+        if (!valid) continue;
+        float* o = reinterpret_cast<float*>(a.out) + grow * a.ldo;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-          if (a.bias) {
-            const float4* bp4 = reinterpret_cast<const float4*>(a.bias + n0);     // bias arrays are padded to the N tile
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) { const float4 b4 = __ldg(bp4 + j / 4); f[j] += b4.x; f[j + 1] += b4.y; f[j + 2] += b4.z; f[j + 3] += b4.w; }
-          }
-          if (a.out_f32) {
-            float* o = reinterpret_cast<float*>(a.out) + grow * a.ldo + n0;
-            if (a.row_stats) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j)
-                if (n0 + j < a.n_valid) row_sum += __expf(f[j] - row_max);   // SFU exp: 256 per thread sit on this tile's critical path
-            }
-            if (n0 + 32 <= a.n_valid && (a.ldo & 3) == 0) {   // 16-byte stores: the row pitch and n0 are multiples of 4 floats
-#pragma unroll
-              for (int j = 0; j < 32; j += 4) {
-                float4 x = make_float4(f[j], f[j + 1], f[j + 2], f[j + 3]);
-                if (a.relu) { x.x = fmaxf(x.x, 0.f); x.y = fmaxf(x.y, 0.f); x.z = fmaxf(x.z, 0.f); x.w = fmaxf(x.w, 0.f); }
-                *reinterpret_cast<float4*>(o + j) = x;
-              }
-            } else if (n0 + 32 <= a.n_valid) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) o[j] = a.relu ? fmaxf(f[j], 0.f) : f[j];
-            } else {
-              for (int j = 0; j < 32 && n0 + j < a.n_valid; ++j) o[j] = a.relu ? fmaxf(f[j], 0.f) : f[j];
-            }
-          } else {
-            __half* o = reinterpret_cast<__half*>(a.out) + grow * a.ldo + n0;
-            if (a.residual) {
-              const uint4* rp = reinterpret_cast<const uint4*>(a.residual + grow * a.ldo + n0);
-#pragma unroll
-              for (int g = 0; g < 4; ++g) {
-                const uint4 rv = __ldg(rp + g);
-                const __half2* h = reinterpret_cast<const __half2*>(&rv);
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  const float2 x = __half22float2(h[j]);
-                  f[g * 8 + 2 * j] += x.x;
-                  f[g * 8 + 2 * j + 1] += x.y;
-                }
-              }
-            }
-            uint4* op = reinterpret_cast<uint4*>(o);
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              uint4 ov;
-              __half2* h = reinterpret_cast<__half2*>(&ov);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                float x0 = f[g * 8 + 2 * j], x1 = f[g * 8 + 2 * j + 1];
-                if (a.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-                if (zero) { x0 = 0.f; x1 = 0.f; }
-                h[j] = __floats2half2_rn(x0, x1);
-              }
-              op[g] = ov;
-            }
-          }
+        for (int j = 0; j < N_TILE / 8; ++j) {
+          const int n = nb + 8 * j;
+          float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+          if (a.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+          if (n + 1 < a.n_valid) *reinterpret_cast<float2*>(o + n) = make_float2(x0, x1);
+          else if (n < a.n_valid) o[n] = x0;
         }
-      }
-      if (a.row_stats && valid) a.row_stats[grow * a.n_tiles + n_tile] = make_float2(row_max, row_sum);
-      umma::tc_fence_before();
-      umma::mbar_arrive(&tempty[acc]);
-    }
-  }
-
-  umma::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    umma::tc_fence_after();
-    umma::tmem_dealloc<C::kTmemCols>(tmem_base);
-  }
-}
-
-// =====================================================================================================
-// CTA-pair variant of the 3x3 convolution (cta_group::2).  ncu on the single-CTA kernel (profiles/r01_*):
-// tensor pipe 56-60 %, L2 40 %, DRAM 6 % -> bound by the 128 B/cycle shared-memory port: per k-block the
-// MMAs read 48 KB of operands while TMA writes another 48 KB.  Here two CTAs of a cluster compute two
-// adjacent M-tiles with ONE tcgen05.mma.cta_group::2 (M = 256): each CTA stages its own A tile and only
-// HALF of the weight tile (N/2 rows), so TMA writes drop to 32 KB and MMA operand reads to 32 KB per
-// k-block per SM, and the smaller stage allows a 6-deep ring.
-// Leader = cluster rank 0: owns the full[] barriers (both CTAs' TMA loads complete_tx there), issues the
-// MMAs, and its tempty[] barriers collect the epilogue arrivals of both CTAs.  tcgen05.commit multicasts
-// to the empty[] / tfull[] barriers of both CTAs.
-constexpr int kStages2 = 5;
-constexpr int kEpiWarps2 = 8;
-constexpr int kStageRow = 36;                                  // floats per staged row (32 + 4 pad: conflict-free both ways)
-constexpr int kEpiStageBytes = kEpiWarps2 * 32 * kStageRow * 4; // 36 KB: one 32x32 fp32 block per epilogue warp
-
-template <int N_TILE>
-struct Cfg2 {
-  static constexpr int kBHalfBytes = (N_TILE / 2) * 128;
-  static constexpr int kStageBytes = kAStageBytes + kBHalfBytes;
-  static constexpr int kTmemCols = Cfg<N_TILE>::kTmemCols;
-  static constexpr int kSmemBytes = kStages2 * kStageBytes + kEpiStageBytes + 256 + 1024;
-  static_assert(N_TILE % 32 == 0 && N_TILE <= 256, "UMMA N constraint for M=256 and an even split of B");
-};
-
-constexpr int kThreads2 = 384;             // warps 0-3: TMA / MMA / TMEM alloc / spare; warps 4-11: epilogue
-
-template <int N_TILE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads2, 1)
-k_igemm2(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Args a) {
-  using C = Cfg2<N_TILE>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  float* epi_stage = reinterpret_cast<float*>(smem + kStages2 * C::kStageBytes);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages2 * C::kStageBytes + kEpiStageBytes);
-  uint64_t* full = bars;                  // [kStages2]  (used in the leader only)
-  uint64_t* empty = bars + kStages2;      // [kStages2]  per CTA, signalled by multicast commit
-  uint64_t* tfull = bars + 2 * kStages2;  // [2]         per CTA, signalled by multicast commit
-  uint64_t* tempty = tfull + 2;           // [2]         leader: 512 arrivals (8 epilogue warps of both CTAs)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = umma::cluster_ctarank();
-  const bool leader = rank == 0;
-
-  if (warp == 0 && lane == 0) {
-    umma::prefetch_tmap(&tmA);
-    umma::prefetch_tmap(&tmB);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStages2; ++s) { umma::mbar_init(&full[s], 1); umma::mbar_init(&empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { umma::mbar_init(&tfull[i], 1); umma::mbar_init(&tempty[i], 512); }
-    umma::fence_barrier_init();
-    umma::fence_proxy_async();
-  }
-  if (warp == 2) umma::tmem_alloc2<C::kTmemCols>(tmem_slot);
-  umma::tc_fence_before();
-  __syncthreads();
-  umma::cluster_sync_all();               // barriers of both CTAs are initialised before any remote arrive / TMA
-  umma::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const int n_kb = a.n_taps * a.k_chunks;
-  const int rows = args_rows(a);
-  const int m_tiles = a.n_dev ? (rows + kTileM - 1) / kTileM : a.m_tiles;
-  const int pairs = (m_tiles + 1) / 2;
-  const int n_clusters = gridDim.x / 2, cluster_id = blockIdx.x / 2;
-
-  if (warp == 0) {
-    // ------------------------------------------------------------ TMA producer (one per CTA)
-    if (lane == 0) {
-      uint32_t it = 0;
-      for (int pair = cluster_id; pair < pairs; pair += n_clusters) {
-        const int m_tile = 2 * pair + (int)rank;
-        // dense mode: first output pixel of this tile as (image, row, column); im2col walks on from there
-        const int pix0 = m_tile * kTileM, img0 = pix0 / 90, row0 = (pix0 % 90) / 9, col0 = pix0 % 9;
-        for (int tap = 0; tap < a.n_taps; ++tap) {
-          const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-          for (int kc = 0; kc < a.k_chunks; ++kc, ++it) {
-            const uint32_t s = it % kStages2, ph = (it / kStages2) & 1;
-            umma::mbar_wait(&empty[s], ph ^ 1);
-            uint8_t* sA = smem + s * C::kStageBytes;
-            uint8_t* sB = sA + kAStageBytes;
-            if (leader) umma::mbar_expect_tx(&full[s], 2u * (a.a_bytes + (uint32_t)C::kBHalfBytes));
-            if (a.conv == 2)
-              umma::tma2_load_im2col_4d(sA, &tmA, &full[s], kc * kBlockK, col0 - 1, row0 - 1, img0, (uint16_t)(dx + 1), (uint16_t)(dy + 1));
-            else
-              umma::tma2_load_3d(sA, &tmA, &full[s], kc * kBlockK, dx, m_tile * a.box_r + dy);
-            umma::tma2_load_2d(sB, &tmB, &full[s], kc * kBlockK, tap * a.n_total + (int)rank * (N_TILE / 2));
-          }
+      } else {
+        if (!valid) continue;
+        __half* o = reinterpret_cast<__half*>(a.out) + grow * a.ldo;
+        const float* r32 = a.residual32 ? a.residual32 + grow * a.ldo : nullptr;
+        const __half* r16 = (!a.residual32 && a.residual) ? a.residual + grow * a.ldo : nullptr;
+        float* o32 = a.out32 ? a.out32 + grow * a.ldo : nullptr;
+#pragma unroll
+        for (int j = 0; j < N_TILE / 8; ++j) {
+          const int n = nb + 8 * j;
+          float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+          if (r32) { const float2 r = __ldg(reinterpret_cast<const float2*>(r32 + n)); x0 += r.x; x1 += r.y; }
+          else if (r16) { const float2 r = __half22float2(__ldg(reinterpret_cast<const __half2*>(r16 + n))); x0 += r.x; x1 += r.y; }
+          if (a.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+          if (zero) { x0 = 0.f; x1 = 0.f; }
+          *reinterpret_cast<__half2*>(o + n) = __floats2half2_rn(x0, x1);
+          if (o32) *reinterpret_cast<float2*>(o32 + n) = make_float2(x0, x1);
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------ MMA issuer (leader CTA only)
-    if (leader && lane == 0) {
-      constexpr uint32_t idesc = umma::idesc_f16(256, N_TILE);
-      uint32_t it = 0, tcount = 0;
-      for (int pair = cluster_id; pair < pairs; pair += n_clusters, ++tcount) {
-        const uint32_t acc = tcount & 1, aph = (tcount >> 1) & 1;
-        umma::mbar_wait(&tempty[acc], aph ^ 1);       // cta-scope acquire: an acquire.cluster wait emits CCTL.IVALL (L1 flush)
-        umma::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * N_TILE;
-        for (int kb = 0; kb < n_kb; ++kb, ++it) {
-          const uint32_t s = it % kStages2, ph = (it / kStages2) & 1;
-          umma::mbar_wait(&full[s], ph);
-          umma::tc_fence_after();
-          const uint32_t sA = umma::smem_u32(smem + s * C::kStageBytes);
-          const uint64_t da = umma::smem_desc_sw128(sA);
-          const uint64_t db = umma::smem_desc_sw128(sA + kAStageBytes);
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k)
-            umma::mma2_f16_ss(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-          umma::mma2_commit_multicast(&empty[s]);
-        }
-        umma::mma2_commit_multicast(&tfull[acc]);
-      }
-    }
-  } else if (warp >= 4) {
-    // ------------------------------------------------------------ epilogue: 8 warps per CTA; warps w and w+4 share a TMEM
-    // lane quarter (w % 4) and split the columns in halves.  TMEM hands every thread one accumulator ROW, but a warp that
-    // loads / stores "one row per lane" touches 32 different 128-byte lines per instruction and saturates L1 (ncu: l1tex
-    // 50-60 % with the fp16 skip stream alone).  Each warp therefore transposes its 32x32 block through a padded
-    // shared-memory tile, so global accesses cover whole lines: 8 lanes per row for fp32, 4 lanes per row for fp16.
-    // Dense pixel layout only (a.conv == 2); the strip layout is served by the single-CTA kernel.
-    const int q = warp & 3;
-    const int half = (warp - 4) >> 2;                        // 0: columns [0, N/2), 1: [N/2, N)
-    float* S = epi_stage + (warp - 4) * 32 * kStageRow;
-    const uint32_t tempty_remote[2] = {umma::mapa_shared(&tempty[0], 0), umma::mapa_shared(&tempty[1], 0)};
-    constexpr int kChunks = N_TILE / 64;                     // 32-column chunks per half
-    const int r4 = lane >> 3, c4 = (lane & 7) * 4;           // fp32 view: rows r4 + 4k, 4 floats at column c4
-    const int r8 = lane >> 2, c8 = (lane & 3) * 8;           // fp16 view: rows r8 + 8k, 8 halves at column c8
-    const int cbeg = half * (N_TILE / 2);
-    uint32_t tcount = 0;
-    // The skip stream of a tile is one contiguous block (kTileM pixels x N channels).  With only a chunk per warp in
-    // flight its loads were DRAM-latency bound (ncu: conv2 with the fp32 stream 17 us per tile vs 14.8 us of MMA), so
-    // one warp pulls the block of the NEXT tile into L2 a whole tile ahead; the chunk loads then hit L2.
-    auto prefetch_skip = [&](int pr) {
-      if (warp != 4 || pr >= pairs || !(a.residual32 || a.residual)) return;
-      const long long row0 = (long long)(2 * pr + (int)rank) * kTileM;
-      const long long nrow = rows - row0 < kTileM ? rows - row0 : kTileM;
-      if (nrow <= 0) return;
-      const size_t esz = a.residual32 ? 4 : 2;
-      const char* base = (a.residual32 ? reinterpret_cast<const char*>(a.residual32) : reinterpret_cast<const char*>(a.residual)) +
-                         (size_t)row0 * a.ldo * esz;
-      const size_t total = (size_t)nrow * a.ldo * esz;           // multiple of 16: ldo is a multiple of 64 channels
-      for (size_t off = (size_t)lane * 16384; off < total; off += 32 * 16384)
-        umma::l2_prefetch_bulk(base + off, (uint32_t)(total - off < 16384 ? total - off : 16384));
-    };
-    prefetch_skip(cluster_id);
-    for (int pair = cluster_id; pair < pairs; pair += n_clusters, ++tcount) {
-      const int m_tile = 2 * pair + (int)rank;
-      const uint32_t acc = tcount & 1, aph = (tcount >> 1) & 1;
-      const long long rbase = (long long)m_tile * kTileM + q * 32;     // first global pixel row of this warp
-      prefetch_skip(pair + n_clusters);
-      const float* r32 = a.residual32 ? a.residual32 + rbase * a.ldo + cbeg : nullptr;
-      const __half* r16 = (!a.residual32 && a.residual) ? a.residual + rbase * a.ldo + cbeg : nullptr;
-      float4 nf[8];                                          // skip stream of the next chunk, line-coalesced
-      uint4 nh[4];
-      auto fetch = [&](int ch) {
-        if (r32) {
-#pragma unroll
-          for (int k = 0; k < 8; ++k)
-            nf[k] = (rbase + r4 + 4 * k < rows) ? __ldg(reinterpret_cast<const float4*>(r32 + (size_t)(r4 + 4 * k) * a.ldo + ch * 32 + c4))
-                                                  : make_float4(0.f, 0.f, 0.f, 0.f);
-        } else if (r16) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            nh[k] = (rbase + r8 + 8 * k < rows) ? __ldg(reinterpret_cast<const uint4*>(r16 + (size_t)(r8 + 8 * k) * a.ldo + ch * 32 + c8))
-                                                  : make_uint4(0u, 0u, 0u, 0u);
-        }
-      };
-      fetch(0);
-      umma::mbar_wait(&tfull[acc], aph);
-      umma::tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + acc * N_TILE + cbeg;
-#pragma unroll 1
-      for (int ch = 0; ch < kChunks; ++ch) {
-        const int c0 = cbeg + ch * 32;
-        // 1. skip stream of this chunk: coalesced registers -> staged tile
-        if (r32) {
-#pragma unroll
-          for (int k = 0; k < 8; ++k) *reinterpret_cast<float4*>(S + (r4 + 4 * k) * kStageRow + c4) = nf[k];
-        } else if (r16) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const __half2* h = reinterpret_cast<const __half2*>(&nh[k]);
-            const float2 f0 = __half22float2(h[0]), f1 = __half22float2(h[1]), f2 = __half22float2(h[2]), f3 = __half22float2(h[3]);
-            float* d = S + (r8 + 8 * k) * kStageRow + c8;
-            *reinterpret_cast<float4*>(d) = make_float4(f0.x, f0.y, f1.x, f1.y);
-            *reinterpret_cast<float4*>(d + 4) = make_float4(f2.x, f2.y, f3.x, f3.y);
-          }
-        }
-        if (ch + 1 < kChunks) fetch(ch + 1);
-        uint32_t v[32];
-        umma::tmem_ld_32x32(t_row + ch * 32, v);
-        __syncwarp();
-        // 2. own row: accumulator + shift (+ skip), ReLU
-        const float4* bp = reinterpret_cast<const float4*>(a.bias + c0);
-        float* own = S + lane * kStageRow;
-#pragma unroll
-        for (int g = 0; g < 8; ++g) {
-          const float4 b = __ldg(bp + g);
-          float4 x = make_float4(__uint_as_float(v[4 * g]) + b.x, __uint_as_float(v[4 * g + 1]) + b.y,
-                                 __uint_as_float(v[4 * g + 2]) + b.z, __uint_as_float(v[4 * g + 3]) + b.w);
-          if (r32 || r16) { const float4 rr = *reinterpret_cast<const float4*>(own + 4 * g); x.x += rr.x; x.y += rr.y; x.z += rr.z; x.w += rr.w; }
-          if (a.relu) { x.x = fmaxf(x.x, 0.f); x.y = fmaxf(x.y, 0.f); x.z = fmaxf(x.z, 0.f); x.w = fmaxf(x.w, 0.f); }
-          *reinterpret_cast<float4*>(own + 4 * g) = x;
-        }
-        __syncwarp();
-        // 3. line-coalesced stores: fp32 copy (next block's skip stream) and fp16 activations (next conv's operand)
-        if (a.out32) {
-          float* o32 = a.out32 + rbase * a.ldo + c0;
-#pragma unroll
-          for (int k = 0; k < 8; ++k)
-            if (rbase + r4 + 4 * k < rows)
-              *reinterpret_cast<float4*>(o32 + (size_t)(r4 + 4 * k) * a.ldo + c4) = *reinterpret_cast<const float4*>(S + (r4 + 4 * k) * kStageRow + c4);
-        }
-        {
-          __half* o16 = reinterpret_cast<__half*>(a.out) + rbase * a.ldo + c0;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const float* sp = S + (r8 + 8 * k) * kStageRow + c8;
-            const float4 x0 = *reinterpret_cast<const float4*>(sp), x1 = *reinterpret_cast<const float4*>(sp + 4);
-            uint4 ov;
-            __half2* oh = reinterpret_cast<__half2*>(&ov);
-            oh[0] = __floats2half2_rn(x0.x, x0.y); oh[1] = __floats2half2_rn(x0.z, x0.w);
-            oh[2] = __floats2half2_rn(x1.x, x1.y); oh[3] = __floats2half2_rn(x1.z, x1.w);
-            if (rbase + r8 + 8 * k < rows) *reinterpret_cast<uint4*>(o16 + (size_t)(r8 + 8 * k) * a.ldo + c8) = ov;
-          }
-        }
-        __syncwarp();
-      }
-      umma::tc_fence_before();
-      umma::mbar_arrive_cluster(tempty_remote[acc]);
-    }
-  }
-
-  umma::tc_fence_before();
-  __syncthreads();
-  umma::cluster_sync_all();               // nobody frees TMEM / exits while the peer may still touch this CTA
-  if (warp == 2) {
-    umma::tc_fence_after();
-    umma::tmem_dealloc2<C::kTmemCols>(tmem_base);
   }
 }
 

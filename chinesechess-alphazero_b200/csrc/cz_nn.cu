@@ -1,10 +1,10 @@
-// cz_nn.cu — policy + value network forward (agent/model.py:32-83) on B200.
+// cz_nn.cu — policy + value network forward (agent/model.py:32-83) on H100 (sm_90a).
 //
 //   packed boards --k_conv_first--> strip activations (5x5 input conv over one-hot planes is a gather-sum
 //                                   of <= 25 weight rows per pixel; plane encoding never materialises)
-//   2 x blocks of  igemm::k_igemm   3x3 conv as implicit GEMM on tcgen05 (BN folded, +skip, ReLU fused)
+//   2 x blocks of  igemm::k_igemm   3x3 conv as implicit GEMM on wgmma (BN folded, +skip, ReLU fused)
 //   k_heads                         1x1 policy/value convs + BN + ReLU, value MLP + tanh
-//   igemm::k_igemm (GEMM mode)      policy_out Dense 360 -> 2086 on tcgen05
+//   igemm::k_igemm (GEMM mode)      policy_out Dense 360 -> 2086 on wgmma
 //   k_softmax                       2086-way softmax
 //
 // BatchNormalization is inference-mode (moving statistics, eps = 1e-3, data/model/model_best_config.json)
@@ -21,7 +21,6 @@
 
 #include "cz_err.h"
 #include "cz_igemm.cuh"
-#include "cz_igemm3.cuh"
 #include "cz_nn.cuh"
 
 namespace cznn {
@@ -111,33 +110,25 @@ static int make_map_2d(CUtensorMap* m, const void* base, int k, long long rows, 
   return 0;
 }
 
-// activation matrix [rows][c] (fp16 or fp32), box {16 columns, 32 rows}: the tiles the conv epilogue loads (skip stream) and
-// stores (outputs) with TMA.  16 fp32 = 64-byte rows -> SWIZZLE_64B, 16 fp16 = 32-byte rows -> SWIZZLE_32B.
-static int make_map_tile32(CUtensorMap* m, const void* base, int c, long long rows, bool f32) {
-  if (load_encode()) return CZ_ERR_CUDA;
-  const cuuint64_t es = f32 ? 4 : 2;
-  cuuint64_t dims[2] = {(cuuint64_t)c, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)c * es};
-  cuuint32_t box[2] = {igemm::kChunkCols3, 32};
-  cuuint32_t est[2] = {1, 1};
-  CUresult r = g_encode(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides,
-                        box, est, CU_TENSOR_MAP_INTERLEAVE_NONE, f32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B,
-                        CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return cz_fail(CZ_ERR_CUDA, "cuTensorMapEncodeTiled(tile32) failed: %d", (int)r);
-  return 0;
-}
-
 static int g_num_sms = 0;
 static int num_sms() {
   if (!g_num_sms) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_num_sms <= 0) g_num_sms = 148;
+    if (g_num_sms <= 0) g_num_sms = 132;
   }
   return g_num_sms;
 }
 
+// Programmatic dependent launch: a conv's CTAs may become resident and run their prologue (barrier init, tensor-map prefetch)
+// while the previous kernel of the stream is still running; griddepcontrol.wait in the kernel orders the data.  CZ_PDL=0
+// launches the plain way.
+static bool use_pdl() {
+  static int pdl = -1;
+  if (pdl < 0) { const char* e = getenv("CZ_PDL"); pdl = (e && e[0] == '0') ? 0 : 1; }
+  return pdl == 1;
+}
 template <int N_TILE>
 static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const igemm::Args& a, cudaStream_t st) {
   using C = igemm::Cfg<N_TILE>;
@@ -149,153 +140,21 @@ static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const 
   const int tiles = a.m_tiles * a.n_tiles;
   if (tiles <= 0) return 0;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  igemm::k_igemm<N_TILE><<<grid, igemm::kThreads, C::kSmemBytes, st>>>(tmA, tmB, a);
-  CZ_CUDA(cudaGetLastError());
-  return 0;
-}
-
-// CTA-pair conv: B tensor map must have box rows = N_TILE / 2
-template <int N_TILE>
-static int launch_igemm2_t(const CUtensorMap& tmA, const CUtensorMap& tmB_half, const igemm::Args& a, cudaStream_t st) {
-  using C = igemm::Cfg2<N_TILE>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    CZ_CUDA(cudaFuncSetAttribute(igemm::k_igemm2<N_TILE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
-    attr_set = true;
-  }
-  const int pairs = (a.m_tiles + 1) / 2;
-  if (pairs <= 0) return 0;
-  const int clusters = pairs < num_sms() / 2 ? pairs : num_sms() / 2;
-  igemm::k_igemm2<N_TILE><<<2 * clusters, igemm::kThreads2, C::kSmemBytes, st>>>(tmA, tmB_half, a);
-  CZ_CUDA(cudaGetLastError());
-  return 0;
-}
-static int launch_igemm2(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB_half, const igemm::Args& a, cudaStream_t st) {
-  switch (n_tile) {
-    case 64: return launch_igemm2_t<64>(tmA, tmB_half, a, st);
-    case 128: return launch_igemm2_t<128>(tmA, tmB_half, a, st);
-    case 192: return launch_igemm2_t<192>(tmA, tmB_half, a, st);
-    case 256: return launch_igemm2_t<256>(tmA, tmB_half, a, st);
-  }
-  return cz_fail(CZ_ERR_UNSUPPORTED, "igemm2: unsupported N tile %d", n_tile);
-}
-// k_igemm3: same mainloop, all-TMA epilogue (cz_igemm3.cuh).  Measured (profiles/r02c_*): +15 % (C=128, no skip) to +41 % (C=128,
-// fp16 skip) and +35 % (C=192) over k_igemm2, equal at C=256 without the fp32 skip stream (tensor pipe 90 %); with the fp32
-// stream (4-deep operand ring beside 96 KB of epilogue tiles, TMA round trips serialised per chunk) it is ~4 % slower in the
-// power-capped 256x20 forward, so that one launch shape keeps k_igemm2.  CZ_EPI=2 / 3 force the old / new epilogue everywhere.
-static int epilogue_choice() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("CZ_EPI"); v = (e && e[0] == '2') ? 2 : (e && e[0] == '3') ? 3 : 0; }
-  return v;
-}
-static bool use_tma_epilogue() { return epilogue_choice() != 2; }
-static bool use_tma_epilogue_for(int c, bool fp32_stream) {
-  if (epilogue_choice() == 2) return false;
-  if (epilogue_choice() == 3) return true;
-  return !(c == 256 && fp32_stream);
-}
-static int g_cluster4 = 0;                 // set by nn_create from CZ_CLUSTER4 (launch_igemm3, C = 256)
-template <int N_TILE, int MT, int PAIRS = 1>
-static int launch_igemm3_t(const CUtensorMap& tmA, const CUtensorMap& tmB_half, const CUtensorMap& tmOut16, const CUtensorMap& tmSkip,
-                           const CUtensorMap& tmOut32, const igemm::Args& a, int skip_mode, bool out32, cudaStream_t st, int n_split = 1) {
-  using C = igemm::Cfg3<N_TILE, MT>;
-  static bool attr_set = false;
-  static int max_clusters = 0;
-  if (!attr_set) {
-    CZ_CUDA(cudaFuncSetAttribute(igemm::k_igemm3<N_TILE, MT, PAIRS>, cudaFuncAttributeMaxDynamicSharedMemorySize, igemm::kSmemLimit3));
-    attr_set = true;
-    max_clusters = num_sms() / (2 * PAIRS);
-    if (PAIRS > 1) {                       // 4-CTA clusters must fit inside a GPC: ask how many can be resident at once
-      cudaLaunchConfig_t oc;
-      memset(&oc, 0, sizeof(oc));
-      oc.gridDim = dim3(2 * PAIRS * max_clusters); oc.blockDim = dim3(igemm::kThreads2); oc.dynamicSmemBytes = igemm::kSmemLimit3;
-      int nc = 0;
-      if (cudaOccupancyMaxActiveClusters(&nc, igemm::k_igemm3<N_TILE, MT, PAIRS>, &oc) == cudaSuccess && nc > 0 && nc < max_clusters) max_clusters = nc;
-      else (void)cudaGetLastError();
-      fprintf(stderr, "[cczero] 4-CTA clusters of k_igemm3<%d, %d>: %d resident at once (%d of %d SMs)\n", N_TILE, MT, max_clusters,
-              4 * max_clusters, num_sms());
-    }
-  }
-  igemm::Args3 p;
-  p.a = a;
-  p.skip_mode = skip_mode; p.out32 = out32 ? 1 : 0; p.n_split = n_split;
-  p.fbytes = (skip_mode == 2 || out32) ? 2048 : (skip_mode == 1 ? 1024 : 0);
-  { static int nf = -1; if (nf < 0) { const char* e = getenv("CZ_NF"); nf = e ? atoi(e) : 3; if (nf < 3) nf = 3; if (nf > igemm::kMaxNF3) nf = igemm::kMaxNF3; } p.nf = nf; }
-  { static int sp = -1; if (sp < 0) { const char* e = getenv("CZ_SPLIT_PROD"); sp = (e && e[0] == '1') ? 1 : 0; } p.split_producer = sp; }
-  p.stages = C::max_stages(p.fbytes, p.nf);
-  { static int cap = -1; if (cap < 0) { const char* e = getenv("CZ_STAGES"); cap = e ? atoi(e) : 0; } if (cap > 1 && cap < p.stages) p.stages = cap; }
-  if (p.stages < 2) return cz_fail(CZ_ERR_UNSUPPORTED, "igemm3: no room for the operand ring");
-  const int pairs = ((a.n_dev ? (a.rows + igemm::kTileM - 1) / igemm::kTileM : a.m_tiles) + 2 * MT - 1) / (2 * MT);
-  if (pairs <= 0) return 0;
-  const int items = (pairs * (n_split > 1 ? n_split : 1) + PAIRS - 1) / PAIRS;     // cluster-level steps
-  const int clusters = items < max_clusters ? items : max_clusters;
-  // Programmatic dependent launch: this conv's CTAs may become resident and run their prologue (barriers, TMEM, tensor map
-  // prefetch) while the previous kernel of the stream is still running; griddepcontrol.wait in the kernel orders the data.
-  // Measured on one box, interleaved (profiles/r02o_*): UCI go depth 8 56.7 -> 54.3 ms, c2 1.521 -> 1.540 M sims/s, c3 equal.
-  // CZ_PDL=0 launches the plain way.
-  static int pdl = -1;
-  if (pdl < 0) { const char* e = getenv("CZ_PDL"); pdl = (e && e[0] == '0') ? 0 : 1; }
-  if (pdl) {
+  if (use_pdl()) {
     cudaLaunchConfig_t lc;
     memset(&lc, 0, sizeof(lc));
-    lc.gridDim = dim3(2 * PAIRS * clusters); lc.blockDim = dim3(igemm::kThreads2);
-    lc.dynamicSmemBytes = C::smem_bytes(p.stages, p.fbytes, p.nf); lc.stream = st;
+    lc.gridDim = dim3(grid); lc.blockDim = dim3(igemm::kThreads); lc.dynamicSmemBytes = C::kSmemBytes; lc.stream = st;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     lc.attrs = at; lc.numAttrs = 1;
-    CZ_CUDA(cudaLaunchKernelEx(&lc, igemm::k_igemm3<N_TILE, MT, PAIRS>, tmA, tmB_half, tmOut16, tmSkip, tmOut32, p));
+    CZ_CUDA(cudaLaunchKernelEx(&lc, igemm::k_igemm<N_TILE>, tmA, tmB, a));
   } else {
-    igemm::k_igemm3<N_TILE, MT, PAIRS><<<2 * PAIRS * clusters, igemm::kThreads2, C::smem_bytes(p.stages, p.fbytes, p.nf), st>>>(tmA, tmB_half, tmOut16, tmSkip, tmOut32, p);
+    igemm::k_igemm<N_TILE><<<grid, igemm::kThreads, C::kSmemBytes, st>>>(tmA, tmB, a);
   }
   CZ_CUDA(cudaGetLastError());
   return 0;
 }
-static int launch_igemm3(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB_half, const CUtensorMap& tmOut16, const CUtensorMap& tmSkip,
-                         const CUtensorMap& tmOut32, const igemm::Args& a, int skip_mode, bool out32, cudaStream_t st) {
-  // two M-tiles per CTA against each weight stage wherever the accumulators fit TMEM (C <= 128); CZ_MT=1 forces the single-tile form
-  static int mt2 = -1;
-  if (mt2 < 0) { const char* e = getenv("CZ_MT"); mt2 = (e && e[0] == '1') ? 0 : 1; }
-  switch (n_tile) {
-    case 64: return mt2 ? launch_igemm3_t<64, 2>(tmA, tmB_half, tmOut16, tmSkip, tmOut32, a, skip_mode, out32, st)
-                        : launch_igemm3_t<64, 1>(tmA, tmB_half, tmOut16, tmSkip, tmOut32, a, skip_mode, out32, st);
-    case 128: return mt2 ? launch_igemm3_t<128, 2>(tmA, tmB_half, tmOut16, tmSkip, tmOut32, a, skip_mode, out32, st)
-                         : launch_igemm3_t<128, 1>(tmA, tmB_half, tmOut16, tmSkip, tmOut32, a, skip_mode, out32, st);
-    case 192: return launch_igemm3_t<192, 1>(tmA, tmB_half, tmOut16, tmSkip, tmOut32, a, skip_mode, out32, st);
-    case 256: {
-      // CZ_CLUSTER4=1 when a network runtime is created (experiment, off by default): two CTA pairs per cluster share every
-      // weight stage by TMA multicast.  Bit-identical results (test_cluster4_weight_multicast); on the pool's B200 it is 1.6 %
-      // SLOWER on the 256x20 forward (profiles/r02y_ab_nn.log) — see DESIGN.md section 3.1.
-      if (g_cluster4) return launch_igemm3_t<256, 1, 2>(tmA, tmB_half, tmOut16, tmSkip, tmOut32, a, skip_mode, out32, st);
-      return launch_igemm3_t<256, 1>(tmA, tmB_half, tmOut16, tmSkip, tmOut32, a, skip_mode, out32, st);
-    }
-  }
-  return cz_fail(CZ_ERR_UNSUPPORTED, "igemm3: unsupported N tile %d", n_tile);
-}
-// Small batches (one game's leaves: the UCI / play_games latency path): 64-column tiles, pairs x C/64 work items, as long as
-// every item gets its own CTA pair in one wave.  tmB_32 = the weight map with 32-row boxes.  CZ_NSPLIT=0 turns it off.
-static bool use_n_split(int n_boards, int c) {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("CZ_NSPLIT"); on = (e && e[0] == '0') ? 0 : 1; }
-  if (!on || c <= 64) return false;
-  const int pairs = ((n_boards * 90 + igemm::kTileM - 1) / igemm::kTileM + 1) / 2;
-  return pairs * (c / 64) <= num_sms() / 2;
-}
-static int launch_igemm3_split(int c, const CUtensorMap& tmA, const CUtensorMap& tmB_32, const CUtensorMap& tmOut16, const CUtensorMap& tmSkip,
-                               const CUtensorMap& tmOut32, const igemm::Args& a, int skip_mode, bool out32, cudaStream_t st) {
-  return launch_igemm3_t<64, 1>(tmA, tmB_32, tmOut16, tmSkip, tmOut32, a, skip_mode, out32, st, c / 64);
-}
-static bool use_im2col() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("CZ_CONV_STRIP"); v = (e && e[0] == '1') ? 0 : 1; }
-  return v == 1;
-}
-static bool use_pair_kernel() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("CZ_IGEMM_1CTA"); v = (e && e[0] == '1') ? 0 : 1; }
-  return v == 1;
-}
-
 static int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, const igemm::Args& a, cudaStream_t st) {
   switch (n_tile) {
     case 64: return launch_igemm_t<64>(tmA, tmB, a, st);
@@ -304,6 +163,21 @@ static int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& t
     case 256: return launch_igemm_t<256>(tmA, tmB, a, st);
   }
   return cz_fail(CZ_ERR_UNSUPPORTED, "igemm: unsupported N tile %d (filters must be 64/128/192/256)", n_tile);
+}
+// Small batches (one game's leaves: the UCI / play_games latency path): 64-column tiles, m_tiles x C/64 work items, as long as
+// they fit one wave of CTAs.  The weight map then has 64-row boxes (map_w_64).  CZ_NSPLIT=0 turns it off.
+static bool use_n_split(int n_boards, int c) {
+  static int on = -1;
+  if (on < 0) { const char* e = getenv("CZ_NSPLIT"); on = (e && e[0] == '0') ? 0 : 1; }
+  if (!on || c <= 64) return false;
+  const int m_tiles = (n_boards * 90 + igemm::kTileM - 1) / igemm::kTileM;
+  return m_tiles * (c / 64) <= num_sms();
+}
+// CZ_CONV_STRIP=1: the strip layout (separator row per board, tiled TMA) instead of the dense layout + im2col TMA
+static bool use_im2col() {
+  static int v = -1;
+  if (v < 0) { const char* e = getenv("CZ_CONV_STRIP"); v = (e && e[0] == '1') ? 0 : 1; }
+  return v == 1;
 }
 
 static igemm::Args conv_args(int n_boards, int c, const float* bias, const __half* residual, __half* out, int relu) {
@@ -316,7 +190,7 @@ static igemm::Args conv_args(int n_boards, int c, const float* bias, const __hal
   return a;
 }
 
-// dense pixel layout [n_boards*90][c] + im2col TMA (CTA-pair kernel only)
+// dense pixel layout [n_boards*90][c] + im2col TMA
 static igemm::Args conv_args_dense(int n_boards, int c, const float* bias, const __half* residual, __half* out, int relu) {
   igemm::Args a = conv_args(n_boards, c, bias, residual, out, relu);
   a.conv = 2; a.rows = n_boards * 90; a.m_tiles = (a.rows + 127) / 128; a.a_bytes = 128 * 128;
@@ -639,7 +513,7 @@ struct NetWeights {
   float *wh, *shifth, *wv1, *bv1, *wv2, *bv2;
   __half* w_pol; float* b_pol;
   CUtensorMap map_wpol;
-  std::vector<CUtensorMap> map_w, map_w_half, map_w_32;
+  std::vector<CUtensorMap> map_w, map_w_64;
   bool ready;
 };
 
@@ -670,13 +544,10 @@ struct NnRuntime {
   // tensor maps
   CUtensorMap map_x, map_t, map_y, map_pf, map_wpol;
   std::vector<CUtensorMap> map_w;
-  std::vector<CUtensorMap> map_w_half;   // box rows = C/2 for the CTA-pair kernel
-  std::vector<CUtensorMap> map_w_32;     // box rows = 32: 64-column tiles of the small-batch launches (use_n_split)
+  std::vector<CUtensorMap> map_w_64;     // box rows = 64: 64-column tiles of the small-batch launches (use_n_split)
   bool fp32_skip;                        // keep the residual (skip) stream in fp32: halves the value error of deep nets, ~+30 % time
   int board_pixels;                      // 99 = strip layout (separator row per board), 90 = dense + im2col TMA
   CUtensorMap imap_x, imap_t, imap_y;    // im2col maps of the three activation buffers (dense layout)
-  CUtensorMap omap_x, omap_t, omap_y;    // 32x32 fp16 tile maps of the same buffers (conv epilogue: TMA stores / fp16 skip loads)
-  CUtensorMap fmap_x32, fmap_y32;        // 32x32 fp32 tile maps of the fp32 skip stream
   // optional CUDA-event timing of the residual-tower launches (bench.py roofline)
   bool profile;
   std::vector<cudaEvent_t> ev;        // pairs, recycled
@@ -689,7 +560,7 @@ static void store_net(NnRuntime* r, int k) {
   NetWeights& n = r->nets[k];
   n.w_first = r->w_first; n.shift_first = r->shift_first; n.w_conv = r->w_conv; n.shift_conv = r->shift_conv;
   n.wh = r->wh; n.shifth = r->shifth; n.wv1 = r->wv1; n.bv1 = r->bv1; n.wv2 = r->wv2; n.bv2 = r->bv2;
-  n.w_pol = r->w_pol; n.b_pol = r->b_pol; n.map_wpol = r->map_wpol; n.map_w = r->map_w; n.map_w_half = r->map_w_half; n.map_w_32 = r->map_w_32;
+  n.w_pol = r->w_pol; n.b_pol = r->b_pol; n.map_wpol = r->map_wpol; n.map_w = r->map_w; n.map_w_64 = r->map_w_64;
   n.ready = r->ready;
 }
 static void select_net(NnRuntime* r, int k) {
@@ -698,7 +569,7 @@ static void select_net(NnRuntime* r, int k) {
   const NetWeights& n = r->nets[k];
   r->w_first = n.w_first; r->shift_first = n.shift_first; r->w_conv = n.w_conv; r->shift_conv = n.shift_conv;
   r->wh = n.wh; r->shifth = n.shifth; r->wv1 = n.wv1; r->bv1 = n.bv1; r->wv2 = n.wv2; r->bv2 = n.bv2;
-  r->w_pol = n.w_pol; r->b_pol = n.b_pol; r->map_wpol = n.map_wpol; r->map_w = n.map_w; r->map_w_half = n.map_w_half; r->map_w_32 = n.map_w_32;
+  r->w_pol = n.w_pol; r->b_pol = n.b_pol; r->map_wpol = n.map_wpol; r->map_w = n.map_w; r->map_w_64 = n.map_w_64;
   r->ready = n.ready;
   r->cur = k;
 }
@@ -782,23 +653,17 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
   // reference's trained 192x10 net), 1 = always, 2 = never
   r->fp32_skip = fp32_skip_mode == 1 || (fp32_skip_mode == 0 && blocks >= 10);
   { const char* e = getenv("CZ_FP32_SKIP"); if (e && e[0] == '1') r->fp32_skip = true; if (e && e[0] == '0') r->fp32_skip = false; }
-  { const char* e = getenv("CZ_CLUSTER4"); g_cluster4 = (e && e[0] == '1') ? 1 : 0; }
   r->profile = false; r->ev_used = 0; r->prof_ms = 0; r->prof_flops = 0; r->prof_launches = 0; r->capturing = false;
   Carver cv{(uint8_t*)workspace, 0, bytes};
   layout(r, cv);
   const int c = filters;
   const long long rows = (long long)max_batch * 11;
   int rc = 0;
-  r->board_pixels = (use_im2col() && use_pair_kernel()) ? 90 : 99;
+  r->board_pixels = use_im2col() ? 90 : 99;
   if (r->board_pixels == 90) {
     rc |= make_map_im2col(&r->imap_x, r->x, c, max_batch);
     rc |= make_map_im2col(&r->imap_t, r->t, c, max_batch);
     rc |= make_map_im2col(&r->imap_y, r->y, c, max_batch);
-    rc |= make_map_tile32(&r->omap_x, r->x, c, (long long)max_batch * 90, false);
-    rc |= make_map_tile32(&r->omap_t, r->t, c, (long long)max_batch * 90, false);
-    rc |= make_map_tile32(&r->omap_y, r->y, c, (long long)max_batch * 90, false);
-    rc |= make_map_tile32(&r->fmap_x32, r->x32, c, (long long)max_batch * 90, true);
-    rc |= make_map_tile32(&r->fmap_y32, r->y32, c, (long long)max_batch * 90, true);
   }
   rc |= make_map_3d(&r->map_x, r->x, c, 9, rows, 9, 14);
   rc |= make_map_3d(&r->map_t, r->t, c, 9, rows, 9, 14);
@@ -808,12 +673,10 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
     select_net(r, net);
     rc |= make_map_2d(&r->map_wpol, r->w_pol, 3 * r->pol_k1, kPolN, 256);
     r->map_w.resize(2 * blocks);
-    r->map_w_half.resize(2 * blocks);
-    r->map_w_32.resize(2 * blocks);
+    r->map_w_64.resize(2 * blocks);
     for (int i = 0; i < 2 * blocks; ++i) {
       rc |= make_map_2d(&r->map_w[i], r->w_conv + (size_t)i * 9 * c * c, c, 9LL * c, c);
-      rc |= make_map_2d(&r->map_w_half[i], r->w_conv + (size_t)i * 9 * c * c, c, 9LL * c, c / 2);
-      rc |= make_map_2d(&r->map_w_32[i], r->w_conv + (size_t)i * 9 * c * c, c, 9LL * c, 32);
+      rc |= make_map_2d(&r->map_w_64[i], r->w_conv + (size_t)i * 9 * c * c, c, 9LL * c, 64);
     }
     store_net(r, net);
   }
@@ -978,11 +841,8 @@ static int fw_tower(NnRuntime* r, int n, const int* n_dev) {
   const bool s32 = dense && r->fp32_skip;
   float *x32 = s32 ? r->x32 : nullptr, *y32 = s32 ? r->y32 : nullptr;
   CUtensorMap *ix = &r->imap_x, *iy = &r->imap_y;
-  CUtensorMap *ox = &r->omap_x, *oy = &r->omap_y;           // fp16 tile maps of x / y
-  CUtensorMap *fx = &r->fmap_x32, *fy = &r->fmap_y32;       // fp32 tile maps of x32 / y32
   __half *x = r->x, *y = r->y;
   CUtensorMap *mx = &r->map_x, *my = &r->map_y;
-  const bool epi3 = dense && use_tma_epilogue();
   for (int i = 0; i < r->blocks; ++i) {
     const size_t wsz = (size_t)c;
     igemm::Args a1 = conv_args(n, c, r->shift_conv + (size_t)(2 * i) * wsz, nullptr, r->t, 1);
@@ -994,22 +854,15 @@ static int fw_tower(NnRuntime* r, int n, const int* n_dev) {
       d2.residual32 = x32; d2.out32 = y32;
       { float* t32 = x32; x32 = y32; y32 = t32; }
       // conv1: x -> t (no skip);  conv2: t (+ skip x or x32) -> y (+ y32)
-      if (epi3 && use_n_split(n, c)) {
-        if (launch_igemm3_split(c, *ix, r->map_w_32[2 * i], r->omap_t, r->omap_t, r->omap_t, d1, 0, false, st)) return CZ_ERR_CUDA;
-        if (launch_igemm3_split(c, r->imap_t, r->map_w_32[2 * i + 1], *oy, s32 ? *fx : *ox, *fy, d2, s32 ? 2 : 1, s32, st)) return CZ_ERR_CUDA;
-      } else {
-      if (epi3 && use_tma_epilogue_for(c, false)) {
-        if (launch_igemm3(c, *ix, r->map_w_half[2 * i], r->omap_t, r->omap_t, r->omap_t, d1, 0, false, st)) return CZ_ERR_CUDA;
-      } else if (launch_igemm2(c, *ix, r->map_w_half[2 * i], d1, st)) return CZ_ERR_CUDA;
-      if (epi3 && use_tma_epilogue_for(c, s32)) {
-        if (launch_igemm3(c, r->imap_t, r->map_w_half[2 * i + 1], *oy, s32 ? *fx : *ox, *fy, d2, s32 ? 2 : 1, s32, st)) return CZ_ERR_CUDA;
-      } else if (launch_igemm2(c, r->imap_t, r->map_w_half[2 * i + 1], d2, st)) return CZ_ERR_CUDA;
-      }
+      const bool split = use_n_split(n, c);
+      const int nt = split ? 64 : c;
+      const std::vector<CUtensorMap>& wm = split ? r->map_w_64 : r->map_w;
+      d1.n_tiles = d2.n_tiles = c / nt;
+      if (launch_igemm(nt, *ix, wm[2 * i], d1, st)) return CZ_ERR_CUDA;
+      if (launch_igemm(nt, r->imap_t, wm[2 * i + 1], d2, st)) return CZ_ERR_CUDA;
       CUtensorMap* ti = ix; ix = iy; iy = ti;
-      ti = ox; ox = oy; oy = ti;
-      ti = fx; fx = fy; fy = ti;
     } else {
-      // strip layout (CZ_CONV_STRIP=1 / CZ_IGEMM_1CTA=1 A-B baselines): host-known batch only
+      // strip layout (CZ_CONV_STRIP=1): host-known batch only
       if (launch_igemm(c, *mx, r->map_w[2 * i], a1, st)) return CZ_ERR_CUDA;
       if (launch_igemm(c, r->map_t, r->map_w[2 * i + 1], a2, st)) return CZ_ERR_CUDA;
     }
@@ -1151,22 +1004,16 @@ int cz_igemm_conv3x3(const void* act_in, const void* w, const float* bias, const
   return launch_igemm(c, ma, mb, a, (cudaStream_t)stream);
 }
 
-// Same convolution on DENSE activations fp16 [n_boards][10][9][c] through the im2col TMA path (CTA-pair kernel).
+// Same convolution on DENSE activations fp16 [n_boards][10][9][c] through the im2col TMA path.
 int cz_igemm_conv3x3_dense(const void* act_in, const void* w, const float* bias, const void* residual, void* act_out,
                            int n_boards, int c, int relu, void* stream) {
   using namespace cznn;
   if (c % 64 || c < 64 || c > 256 || n_boards <= 0) return cz_fail(CZ_ERR_ARG, "cz_igemm_conv3x3_dense: bad shape");
   CUtensorMap ma, mb;
   if (make_map_im2col(&ma, act_in, c, n_boards)) return CZ_ERR_CUDA;
-  if (make_map_2d(&mb, w, c, 9LL * c, c / 2)) return CZ_ERR_CUDA;
+  if (make_map_2d(&mb, w, c, 9LL * c, c)) return CZ_ERR_CUDA;
   igemm::Args a = conv_args_dense(n_boards, c, bias, (const __half*)residual, (__half*)act_out, relu);
-  if (use_tma_epilogue()) {
-    CUtensorMap mo, ms;
-    if (make_map_tile32(&mo, act_out, c, (long long)n_boards * 90, false)) return CZ_ERR_CUDA;
-    if (make_map_tile32(&ms, residual ? residual : act_out, c, (long long)n_boards * 90, false)) return CZ_ERR_CUDA;
-    return launch_igemm3(c, ma, mb, mo, ms, mo, a, residual ? 1 : 0, false, (cudaStream_t)stream);
-  }
-  return launch_igemm2(c, ma, mb, a, (cudaStream_t)stream);
+  return launch_igemm(c, ma, mb, a, (cudaStream_t)stream);
 }
 
 // out[m][n] = sum_k a[m][k] * w[n][k] + bias[n]; a fp16 [m_alloc >= ceil128(m)][k], w fp16 [n_pad][k], k % 64 == 0,

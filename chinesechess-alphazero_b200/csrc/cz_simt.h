@@ -2,7 +2,7 @@
 //
 // The kernels are written warp-per-game: 32 lanes cooperate on one board or one
 // search tree, control flow around every collective is warp-uniform, and there is
-// no inter-warp communication.  On the device (nvcc, sm_100a) the primitives map
+// no inter-warp communication.  On the device (nvcc, sm_90a) the primitives map
 // 1:1 to __shfl_sync / __ballot_sync / __syncwarp.  With -DCZ_EMUL the very same
 // kernel source is compiled by g++ against tests/simt_emul/ (32 fibers per warp on
 // one OS thread) so the CPU-only test tier can single-step device logic.  The

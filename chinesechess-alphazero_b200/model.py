@@ -85,7 +85,7 @@ class CChessModel:
         k = getattr(mc, "cnn_filter_size", 3)
         depth = getattr(mc, "input_depth", 14)        # 28 = the use_history network (data/model/model_128_l1_config.json)
         if first != 5 or k != 3 or depth not in (14, 28):
-            raise NotImplementedError("the B200 path implements the 5x5 -> 3x3 residual tower on 14 or 28 input planes")
+            raise NotImplementedError("the GPU path implements the 5x5 -> 3x3 residual tower on 14 or 28 input planes")
         conv(f"input_conv-{first}-{f}", first, depth, f)
         bn("input_batchnorm", f)
         for i in range(1, blocks + 1):

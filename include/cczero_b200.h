@@ -1,4 +1,4 @@
-/* cczero_b200.h — C-ABI of libcczero_b200.so, the B200-native Xiangqi self-play hot path.
+/* cczero_b200.h — C-ABI of libcczero_b200.so, the H100-native Xiangqi self-play hot path.
  *
  * The reference (NeymarL/ChineseChess-AlphaZero) is pure Python and has no FFI; the hot path
  * sits behind three Python surfaces (SURVEY.md §8b).  This header is what a ctypes binding of

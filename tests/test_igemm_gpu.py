@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM kernel vs a plain PyTorch fp32 reference of the same op (GPU only)."""
+"""wgmma implicit-GEMM kernel vs a plain PyTorch fp32 reference of the same op (GPU only)."""
 import ctypes as C
 
 import pytest

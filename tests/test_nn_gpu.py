@@ -78,7 +78,7 @@ def test_forward_chunks_and_batch_of_one(cuda_lib, cuda_env):
 
 @pytest.mark.parametrize("filters,blocks,fp32_skip", [(128, 7, None), (192, 10, None), (256, 20, None), (256, 3, False)])
 def test_small_batch_tiles_equal_full_width_tiles(cuda_lib, cuda_env, filters, blocks, fp32_skip):
-    """A few positions (one game's leaves: UCI / play_games) run the residual convs as 64-column tiles spread over many CTA pairs
+    """A few positions (one game's leaves: UCI / play_games) run the residual convs as 64-column tiles spread over many CTAs
     (cz_nn.cu use_n_split); the same positions inside a batch of 1024 run the full-width tiles.  The K order of every output is the
     same, so policy and value agree bit for bit, and both keep the 1e-3 bound."""
     w = om.init_weights(filters, blocks, 256, seed=3, trained_like=True, spread=0.1)
@@ -98,33 +98,6 @@ def test_small_batch_tiles_equal_full_width_tiles(cuda_lib, cuda_env, filters, b
     ref_p, ref_v = om.forward(w, np.stack([osenv.state_to_planes(s) for s in states]), blocks)
     assert np.abs(p_s.cpu().numpy() - ref_p).max() < 1e-3 and np.abs(v_s.cpu().numpy() - ref_v).max() < 1e-3
     small.close(); big.close()
-
-
-def test_cluster4_weight_multicast(cuda_lib, cuda_env, monkeypatch):
-    """Experiment kept behind CZ_CLUSTER4=1 (cz_igemm3.cuh, PAIRS = 2): the two CTA pairs of a 4-CTA cluster share every weight
-    stage of the 256-wide conv by TMA multicast.  Same K order per output: policy and value bit for bit those of the default launch,
-    odd numbers of tiles included (the second pair then walks an all-out-of-bounds tile)."""
-    w = om.init_weights(256, 3, 256, seed=9, trained_like=True, spread=0.1)
-    states = [osenv.INIT_STATE] + midgame_states(12, 17, lo=1, hi=100)
-    boards = cuda_env.boards_from_states(states)
-    out = {}
-    for mode in ("0", "1"):                                   # the switch is read when a network runtime is created
-        monkeypatch.setenv("CZ_CLUSTER4", mode)
-        for batch in (302, 1024, 1027):      # 302 boards = 107 pair-tiles: odd
-            eng = _engine(cuda_lib, 256, 3, batch, False)     # fp16 skip stream: both convs of a block run the TMA-epilogue kernel
-            eng.set_weights({k: torch.as_tensor(v) for k, v in w.items()})
-            reps = (batch + len(states) - 1) // len(states)
-            p, v = eng.nn_forward_boards(boards.repeat(reps, 1)[:batch])
-            torch.cuda.synchronize()
-            out[(mode, batch)] = (p.clone(), v.clone())
-            eng.close()
-    monkeypatch.setenv("CZ_CLUSTER4", "0")
-    _engine(cuda_lib, 64, 1, 4).close()                       # leave the process-wide switch off for the tests that follow
-    for batch in (302, 1024, 1027):      # 302 boards = 107 pair-tiles: odd
-        assert torch.equal(out[("0", batch)][0], out[("1", batch)][0]) and torch.equal(out[("0", batch)][1], out[("1", batch)][1])
-    ref_p, ref_v = om.forward(w, np.stack([osenv.state_to_planes(s) for s in states]), 3)
-    n = len(states)
-    assert np.abs(out[("1", 1024)][0][:n].cpu().numpy() - ref_p).max() < 1e-3 and np.abs(out[("1", 1024)][1][:n].cpu().numpy() - ref_v).max() < 1e-3
 
 
 @pytest.mark.parametrize("filters,blocks,trained", [(128, 7, False), (192, 4, True)])

@@ -1,7 +1,11 @@
-"""Pin the oracle restatements to the REAL reference (read-only tree at /root/reference).  These tests run in the build
-container; on the GPU box the tree is absent and they skip — the committed golden vectors (tests/golden/, generated from
-the same reference by oracle/gen_golden*.py) carry the pin there."""
-import random
+"""Pin the oracle restatements to the REAL reference.  What the reference computed for every input below is stored in
+tests/golden/reference_pins.json.gz (oracle/gen_golden_pins.py runs the reference to write it), so these comparisons run
+anywhere.  The tests marked `live` execute the reference's own code against the drop-in modules (its worker loops, model
+API, UCI front end and player); they need the reference tree (oracle/ref_import.py) and skip without it."""
+import functools
+import gzip
+import json
+import os
 
 import numpy as np
 import pytest
@@ -9,34 +13,48 @@ import pytest
 from oracle import player as op
 from oracle import ref_import
 from oracle import senv as o
+from oracle.gen_golden_pins import array_digest, planes_digest
 
-pytestmark = pytest.mark.skipif(not ref_import.available(), reason="reference tree not present")
+live = pytest.mark.skipif(not ref_import.available(), reason="reference tree not present")
+
+
+@functools.lru_cache(maxsize=1)
+def pins():
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_pins.json.gz")
+    with gzip.open(path, "rt") as f:
+        return json.load(f)
+
+
+def _json(x):
+    return json.loads(json.dumps(x))          # tuples -> lists, as stored
+
+
+def _check_position(row):
+    s = row["s"]
+    assert o.get_legal_moves(s) == row["lm"], s
+    assert _json(o.done(s)) == row["done"] and _json(o.done(s, need_check=True)) == row["done_check"], s
+    assert planes_digest(o.state_to_planes(s)) == row["planes"], s
+    assert o.has_attack_chessman(s) == row["attack"] and o.fliped_state(s) == row["flip"], s
+    if "m" in row:
+        m = row["m"]
+        assert _json(o.new_step(s, m)) == row["new_step"], (s, m)
+        if "wcc" in row:
+            assert _json(o.will_check_or_catch(s, m)) == row["wcc"], (s, m)
+            assert _json(o.be_catched(s, m)) == row["catched"], (s, m)
 
 
 def test_env_restatement_on_random_playouts():
-    r = ref_import.senv()
-    lt = ref_import.lookup_tables()
-    assert o.ActionLabelsRed == lt.ActionLabelsRed
-    assert [o.flip_move(m) for m in o.ActionLabelsRed[:50]] == [lt.flip_move(m) for m in lt.ActionLabelsRed[:50]]
-    rng = random.Random(7)
+    g = pins()
+    assert o.ActionLabelsRed == g["labels"]
+    assert [o.flip_move(m) for m in o.ActionLabelsRed[:50]] == g["flip50"]
     n = 0
-    for g in range(25):
-        s = r.INIT_STATE
-        for ply in range(200):
-            lm = r.get_legal_moves(s)
-            assert o.get_legal_moves(s) == lm
-            assert o.done(s) == r.done(s) and o.done(s, need_check=True) == r.done(s, need_check=True)
-            assert (o.state_to_planes(s) == r.state_to_planes(s)).all()
-            assert o.has_attack_chessman(s) == r.has_attack_chessman(s) and o.fliped_state(s) == r.fliped_state(s)
-            if r.done(s)[0]:
-                break
-            m = rng.choice(lm)
-            if ply % 2 == 0:
-                assert o.will_check_or_catch(s, m) == r.will_check_or_catch(s, m)
-                assert o.be_catched(s, m) == r.be_catched(s, m)
-            assert o.new_step(s, m) == r.new_step(s, m)
-            s = r.step(s, m)
-            n += 1
+    for game in g["playouts"]:
+        assert game[0]["s"] == o.INIT_STATE
+        for row, nxt in zip(game, game[1:] + [None]):
+            _check_position(row)
+            if nxt is not None:
+                assert o.step(row["s"], row["m"]) == nxt["s"]
+                n += 1
     assert n > 500
 
 
@@ -52,11 +70,9 @@ def test_reference_smoke_vectors():
 
 def test_fen_helpers_match_reference():
     from cczero_b200 import env as penv
-    r = ref_import.senv()
-    s = '4s4/9/4e4/p8/2e2R2p/P5E2/8P/9/9/4S1E2'
-    for st, t in ((o.INIT_STATE, 0), (o.step(o.INIT_STATE, '0001'), 1), (s, 7), (s, 10)):
-        assert o.state_to_fen(st, t) == r.state_to_fen(st, t) == penv.state_to_fen(st, t)
-        assert o.fen_to_state(r.state_to_fen(st, t)) == r.fen_to_state(r.state_to_fen(st, t))
+    for st, t, fen, back in pins()["fen"]:
+        assert o.state_to_fen(st, t) == fen == penv.state_to_fen(st, t)
+        assert o.fen_to_state(fen) == back
 
 
 def _oracle_root(state, sims, k, seed):
@@ -69,25 +85,23 @@ def _oracle_root(state, sims, k, seed):
 
 
 def test_player_restatement_equals_real_player_k1():
-    from oracle.ref_player_harness import real_player_moves
-    for sims, seed in ((80, 1), (150, 2)):
-        real = real_player_moves([(o.INIT_STATE, 0, None, False)], sims, seed)[0]
-        a, node = _oracle_root(o.INIT_STATE, sims, 1, seed)
-        got = {m: (int(e.n), float(e.w), float(e.q), float(e.p)) for m, e in node.a.items()}
-        assert a == real[0] and got == real[1] and node.sum_n == real[2]
+    for real in pins()["player_k1"]:
+        a, node = _oracle_root(o.INIT_STATE, real["sims"], 1, real["seed"])
+        got = {m: [int(e.n), float(e.w), float(e.q), float(e.p)] for m, e in node.a.items()}
+        assert a == real["action"] and got == real["edges"] and node.sum_n == real["sum_n"]
 
 
 def test_canonical_schedule_is_statistically_the_threaded_player_k10():
     """search_threads = 10: the real player is a racy thread pool (not reproducible); the canonical schedule must be
     statistically indistinguishable from it.  Total-variation distance between root visit distributions: oracle-vs-real
     must not exceed the real player's own run-to-run spread, and the seed-averaged distributions must agree."""
-    from oracle.ref_player_harness import real_player_moves
-    sims, k, seeds = 300, 10, range(5)
+    g = pins()["player_k10"]
+    sims, k, seeds = g["sims"], g["search_threads"], range(len(g["visits"]))
     lm = o.get_legal_moves(o.INIT_STATE)
+    assert lm == g["moves"]
 
     def real(seed):
-        r = real_player_moves([(o.INIT_STATE, 0, None, False)], sims, seed, search_threads=k)[0]
-        return np.array([r[1].get(m, (0,))[0] for m in lm], float)
+        return np.array(g["visits"][seed], float)
 
     def mine(seed):
         _, node = _oracle_root(o.INIT_STATE, sims, k, seed)
@@ -111,18 +125,20 @@ def test_game_loop_restatements_replay_live_reference_games():
     from oracle import arena as oarena
     from oracle import ref_worker_harness as h
     from oracle import selfplay as osp
-    play = dict(max_game_length=20, tau_decay_rate=0.98, noise_eps=0.25, enable_resign_rate=0.1, resign_threshold=-0.5, min_resign_turn=4)
+    gold = pins()["game_loops"]
+    assert gold["play"] == dict(max_game_length=20, tau_decay_rate=0.98, noise_eps=0.25, enable_resign_rate=0.1, resign_threshold=-0.5,
+                                min_resign_turn=4)
     pc = op.PlayConfig(simulation_num_per_move=16, search_threads=1, c_puct=1.5, noise_eps=0.25, dirichlet_alpha=0.2,
                        tau_decay_rate=0.98, virtual_loss=3, resign_threshold=-0.5, min_resign_turn=4)
-    for seed in (41, 42):
-        g = h.real_selfplay_game(seed, 16, **play)
+    for g in gold["selfplay"]:
+        seed = g["seed"]
         random.seed(seed)
         np.random.seed(seed)
         r = osp.play_game(pc, op.fake_evaluate_states, h.ReferenceDraws(), max_game_length=20, enable_resign_rate=0.1)
         assert (r["turns"], r["value_red"], r["store"], r["final_state"]) == (g["turns"], g["value_red"], g["store"], g["final_state"])
         assert g["moves"] is None or g["moves"] == r["moves"]
-    for seed, idx in ((43, 0), (44, 1)):
-        g = h.real_arena_game(seed, idx, 16, **play)
+    for g in gold["arena"]:
+        seed, idx = g["seed"], g["idx"]
         random.seed(seed)
         np.random.seed(seed)
         d = h.ReferenceDraws()
@@ -130,6 +146,7 @@ def test_game_loop_restatements_replay_live_reference_games():
         assert (r["turns"], r["value_red"]) == (g["turns"], g["value_red"]) and r["moves"][:len(g["moves"])] == g["moves"]
 
 
+@live
 @pytest.mark.filterwarnings("ignore::DeprecationWarning")          # api.py:68 float(array) under numpy 2
 def test_drop_in_player_searches_through_the_real_model_api(emul_lib):
     """The reference's own CChessModelAPI (agent/api.py:16-74, unmodified; a stand-in object plays the Keras model) serves
@@ -175,31 +192,23 @@ def test_drop_in_player_searches_through_the_real_model_api(emul_lib):
 def test_expanding_data_matches_the_real_trainer_side(emul_env):
     """records.expanding_data vs the reference's worker/optimize.py:234-281 (unmodified; Keras imports stubbed) on one
     golden game record, 14 and 28 planes."""
-    import gzip
-    import json
-    import os
-    from oracle import ref_worker_harness as h
     from cczero_b200.records import expanding_data, record_to_play_data
-    h.worker_modules()
-    import cchess_alphazero.worker.optimize as ropt
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     with gzip.open(os.path.join(root, "tests", "golden", "games_k1.json.gz"), "rt") as f:
         game = next(g for g in json.load(f)["games"] if g["kind"] == "selfplay" and g["result"]["moves"] and g["result"]["value_red"] != 0)
     data = record_to_play_data({"moves": game["result"]["moves"], "value_red": game["result"]["value_red"]})
     for use_history in (False, True):
-        rs, rp, rv = ropt.expanding_data(data, use_history)
-        s, p, v = expanding_data(data, emul_env, use_history=use_history)
-        assert s.shape == rs.shape and (s == rs).all() and (p == rp).all() and (v == rv).all()
+        want = pins()["expanding_data"][str(int(use_history))]
+        assert [array_digest(x) for x in expanding_data(data, emul_env, use_history=use_history)] == want
 
 
+@live
 def test_network_restatement_matches_the_shipped_keras_graph():
-    """oracle/model.py (restated from agent/model.py) vs the layer graph Keras itself wrote for the shipped networks
-    (data/model/model_best_config.json + model_best_weight.h5; model_128_l1_config.json = the 28-plane variant), executed
-    by oracle/keras_graph.py."""
-    import os
+    """oracle/model.py (restated from agent/model.py) vs the layer graph Keras itself wrote for the shipped network
+    (data/model/model_best_config.json + the 30 MB model_best_weight.h5), executed by oracle/keras_graph.py."""
     from cczero_b200.keras_h5 import read_keras_weights
     from oracle import keras_graph, model as om
-    from tests.search_checks import game_history, midgame_states
+    from tests.search_checks import midgame_states
     mdir = os.path.join(ref_import.REF_ROOT, "data", "model")
     w = read_keras_weights(os.path.join(mdir, "model_best_weight.h5"))
     states = [o.INIT_STATE] + midgame_states(11, 4, lo=2, hi=110)
@@ -208,36 +217,31 @@ def test_network_restatement_matches_the_shipped_keras_graph():
     rp, rv = om.forward(w, planes, 10)
     assert gp.shape == (12, 2086) and np.abs(gp - rp).max() < 2e-6 and np.abs(gv[:, 0] - rv).max() < 2e-6
     assert gp.max() > 0.2                                        # a trained, peaked policy - not a degenerate comparison
-    # the 28-plane variant (Input (28,10,9), 7 blocks x 128): random weights under the names of that config
-    # (that legacy file keeps the head widths of an earlier model version: 32 policy / 4 value channels)
+
+
+def test_network_restatement_matches_the_keras_graph_28_planes():
+    """The 28-plane variant (data/model/model_128_l1_config.json: Input (28,10,9), 7 blocks x 128; that legacy file keeps the
+    head widths of an earlier model version, 32 policy / 4 value channels) with random weights under its names: oracle/model.py
+    vs what oracle/keras_graph.py computed from the Keras layer graph of that config."""
+    from oracle import model as om
+    from tests.search_checks import game_history
     w28 = om.init_weights(128, 7, 256, seed=2, trained_like=True, spread=0.5, in_planes=28, policy_filters=32, value_filters=4)
     hists = [game_history(n, 30 + n) for n in (2, 5, 17, 40)]
     p28 = np.stack([o.state_history_to_planes(h[-1], h) for h in hists])
-    gp, gv = keras_graph.run(os.path.join(mdir, "model_128_l1_config.json"), w28, p28)
+    g = pins()["keras_graph_28"]
     rp, rv = om.forward(w28, p28, 7)
-    assert np.abs(gp - rp).max() < 2e-6 and np.abs(gv[:, 0] - rv).max() < 2e-6
+    assert np.abs(np.array(g["policy"]) - rp).max() < 2e-6 and np.abs(np.array(g["value"]) - rv).max() < 2e-6
 
 
 def test_evaluator_tally_matches_the_real_worker():
     """EvaluateWorker.start's win / draw / fail bookkeeping and score (evaluator.py:93-145, unmodified) over canned game
     results vs cczero_b200.evaluator.tally_games."""
-    from oracle import ref_worker_harness as h
     from cczero_b200.evaluator import tally_games
-    _, ev = h.worker_modules()
-    cfg = ref_import.config("mini")
-    results = [1, -1, 0, 1, 1, -1, 0, 0, -1, 1, 1, -1]
-    cfg.eval.game_num = len(results)
-    w = ev.EvaluateWorker(cfg, pid=0)
-    w.start_game = lambda idx: (results[idx], 40)
-    sleep = ev.sleep
-    ev.sleep = lambda s: None
-    try:
-        want = w.start()
-    finally:
-        ev.sleep = sleep
-    assert tuple(want) == tuple(tally_games(list(enumerate(results))))
+    g = pins()["tally"]
+    assert list(g["want"]) == list(tally_games(list(enumerate(g["results"]))))
 
 
+@live
 def test_reference_game_loops_drive_the_drop_in_player(emul_lib):
     """INTEGRATION.md §3, literally: the name `CChessPlayer` inside the reference's worker modules is rebound to
     cczero_b200.player.CChessPlayer and the UNMODIFIED SelfPlayWorker.start_game / EvaluateWorker.start_game play whole
@@ -269,6 +273,7 @@ def test_reference_game_loops_drive_the_drop_in_player(emul_lib):
     assert done >= 8
 
 
+@live
 def test_reference_uci_front_end_drives_the_drop_in_player(emul_lib):
     """The REAL uci.UCI class with `CChessPlayer` rebound to the drop-in: the golden session (recorded with the real
     player) must come out line for line."""
@@ -329,6 +334,7 @@ def test_reference_uci_front_end_drives_the_drop_in_player(emul_lib):
             s.close()
 
 
+@live
 def test_reference_player_runs_on_the_drop_in_rules_engine(emul_env):
     """The other import swap of INTEGRATION.md §3: `senv` inside the reference's agent/player.py rebound to
     cczero_b200.env.StaticEnv - the REAL player must search exactly as it does on its own static_env."""
@@ -353,14 +359,8 @@ def test_reference_player_runs_on_the_drop_in_rules_engine(emul_env):
 def test_env_restatement_on_arbitrary_boards():
     """Unreachable positions (random pieces on random squares, piece counts no game can have): oracle == real static_env."""
     from tests.env_checks import EXTREME_STATES, random_boards
-    r = ref_import.senv()
-    for s in random_boards(600, 5) + [x for x in EXTREME_STATES if 's' in x and 'S' in x]:
-        lm = r.get_legal_moves(s)
-        assert o.get_legal_moves(s) == lm, s
-        assert o.done(s) == r.done(s) and o.done(s, need_check=True) == r.done(s, need_check=True), s
-        assert (o.state_to_planes(s) == r.state_to_planes(s)).all() and o.has_attack_chessman(s) == r.has_attack_chessman(s)
-        if lm and not r.done(s)[0]:
-            m = lm[len(s) % len(lm)]
-            assert o.new_step(s, m) == r.new_step(s, m), (s, m)
-            assert o.will_check_or_catch(s, m) == r.will_check_or_catch(s, m), (s, m)
-            assert o.be_catched(s, m) == r.be_catched(s, m), (s, m)
+    states = random_boards(600, 5) + [x for x in EXTREME_STATES if 's' in x and 'S' in x]
+    rows = pins()["boards"]
+    assert [r["s"] for r in rows] == states
+    for row in rows:
+        _check_position(row)

@@ -9,19 +9,13 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 VARIANTS = {
-    "igemm2 (round-1 epilogue)": {"CZ_EPI": "2"},
-    "auto (igemm3; igemm2 for C=256 fp32 skip)": {},
-    "igemm3 everywhere, nf=3": {"CZ_EPI": "3", "CZ_NF": "3"},
-    "igemm3 everywhere, nf=4": {"CZ_EPI": "3", "CZ_NF": "4"},
-    "auto, one M-tile per CTA at C<=128": {"CZ_MT": "1"},
-    "skip default (fp32 copy of the residual stream beyond 10 blocks)": {},
-    "conv2 on igemm3": {"CZ_EPI": "3"},
-    "cluster4: two CTA pairs per cluster share the weight stages (conv1)": {"CZ_CLUSTER4": "1"},
-    "cluster4 + conv2 on igemm3": {"CZ_CLUSTER4": "1", "CZ_EPI": "3"},
+    "default": {},
+    "no programmatic dependent launch": {"CZ_PDL": "0"},
+    "no 64-column tiles for small batches": {"CZ_NSPLIT": "0"},
     "skip fp16 only (upper bound: breaks 1e-3 at 20 blocks)": {"CZ_FP32_SKIP": "0"},
 }
 SHAPES = [(256, 20, 8192, 3.0), (128, 7, 2048, 1.5), (192, 10, 4096, 1.5)]
-if os.environ.get("AB_ONLY"):                      # e.g. AB_ONLY="auto,one M-tile" AB_SHAPES=small
+if os.environ.get("AB_ONLY"):                      # e.g. AB_ONLY="default,no programmatic" AB_SHAPES=small
     keep = [k.strip() for k in os.environ["AB_ONLY"].split(",")]
     VARIANTS = {k: v for k, v in VARIANTS.items() if any(k.startswith(p) for p in keep)}
 if os.environ.get("AB_SHAPES") == "c3":

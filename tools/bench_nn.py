@@ -43,7 +43,7 @@ def main():
         useful = 2.0 * nb * 90 * 9 * c * c
         issued = 2.0 * ((nb * 11 + 13) // 14) * 128 * 9 * c * c
         print(f"conv3x3 C={c} boards={nb}: {ms:.3f} ms  useful {useful / ms / 1e9:.1f} TFLOP/s  issued {issued / ms / 1e9:.1f} TFLOP/s")
-    # the product kernel: CTA-pair conv on dense activations (im2col TMA), without / with the fp16 skip stream
+    # the product kernel: wgmma conv on dense activations (im2col TMA), without / with the fp16 skip stream
     for c, nb in ((256, 8192), (256, 4096), (128, 2048), (128, 8192), (192, 4096)):
         x = torch.randn(nb, 10, 9, c, device="cuda").half()
         w = (torch.randn(9, c, c, device="cuda") * 0.02).half()
