@@ -981,6 +981,48 @@ int nn_forward_leaves(NnRuntime* r, int net, int part, const uint8_t* boards, in
 void nn_set_capturing(NnRuntime* r, bool on) { if (r) r->capturing = on; }
 bool nn_profiling(const NnRuntime* r) { return r && r->profile; }
 void nn_set_stream(NnRuntime* r, void* stream) { if (r) r->stream = (cudaStream_t)stream; }
+// Parity tests: copy rows of an intermediate buffer out after a forward.  Which physical buffer holds a stage follows the
+// ping-pong of fw_tower and the choice fw_heads makes (x <-> y once per block, the fp32 copies alongside).  Off the forward
+// path: nothing here runs unless a test asks.
+int nn_read_buffer(NnRuntime* r, int which, int n, void* dst, long long dst_bytes, long long* row_bytes) {
+  if (!r) return cz_fail(CZ_ERR_STATE, "cz_nn_read_buffer: engine has no network");
+  if (r->board_pixels != 90) return cz_fail(CZ_ERR_UNSUPPORTED, "cz_nn_read_buffer: strip layout (CZ_CONV_STRIP=1)");
+  const bool s32 = r->fp32_skip, odd = (r->blocks & 1) != 0;
+  const long long act = 90LL * r->filters;
+  const void* src = nullptr;
+  long long row = 0;
+  switch (which) {
+    case CZ_NN_BUF_FIRST_OUT:
+    case CZ_NN_BUF_FIRST_OUT32:
+      if (r->blocks != 1) return cz_fail(CZ_ERR_STATE, "cz_nn_read_buffer: the first convolution's output survives only a 1-block tower");
+      if (which == CZ_NN_BUF_FIRST_OUT32 && !s32) return cz_fail(CZ_ERR_STATE, "cz_nn_read_buffer: no fp32 skip stream");
+      src = which == CZ_NN_BUF_FIRST_OUT ? (const void*)r->x : (const void*)r->x32;
+      row = which == CZ_NN_BUF_FIRST_OUT ? act * 2 : act * 4;
+      break;
+    case CZ_NN_BUF_LAST_CONV1:
+      if (r->blocks < 1) return cz_fail(CZ_ERR_STATE, "cz_nn_read_buffer: no residual block");
+      src = r->t; row = act * 2;
+      break;
+    case CZ_NN_BUF_TOWER_OUT:
+      src = odd ? r->y : r->x; row = act * 2;
+      break;
+    case CZ_NN_BUF_TOWER_OUT32:
+      if (!s32) return cz_fail(CZ_ERR_STATE, "cz_nn_read_buffer: no fp32 skip stream");
+      src = odd ? r->y32 : r->x32; row = act * 4;
+      break;
+    case CZ_NN_BUF_POL_FEAT: src = r->pol_feat; row = 3LL * r->pol_k1 * 2; break;
+    case CZ_NN_BUF_LOGITS: src = r->logits; row = (long long)kPolN * 4; break;
+    case CZ_NN_BUF_STATS: src = r->stats; row = (long long)(kPolN / 256) * 8; break;
+    default: return cz_fail(CZ_ERR_ARG, "cz_nn_read_buffer: unknown buffer %d", which);
+  }
+  if (row_bytes) *row_bytes = row;
+  if (!dst) return 0;
+  if (n < 0 || n > r->max_batch) return cz_fail(CZ_ERR_ARG, "cz_nn_read_buffer: %d rows of a batch of at most %d", n, r->max_batch);
+  if (dst_bytes < (long long)n * row) return cz_fail(CZ_ERR_ARG, "cz_nn_read_buffer: %lld bytes < %d rows x %lld", dst_bytes, n, row);
+  CZ_CUDA(cudaMemcpyAsync(dst, src, (size_t)n * row, cudaMemcpyDeviceToDevice, r->stream));
+  CZ_CUDA(cudaStreamSynchronize(r->stream));
+  return 0;
+}
 int nn_launches_per_forward(const NnRuntime* r) { return r ? 1 + 2 * r->blocks + 3 : 0; }
 double nn_tower_flops_per_position(const NnRuntime* r) { return r ? 2.0 * 90.0 * 9.0 * r->filters * r->filters * 2.0 * r->blocks : 0.0; }
 

@@ -38,5 +38,7 @@ void nn_set_stream(NnRuntime*, void* stream);
 uint64_t nn_launches(const NnRuntime*);
 void nn_profile(NnRuntime*, bool on);
 int nn_profile_read(NnRuntime*, double* ms, uint64_t* launches, double* flops);
+// cz_nn_read_buffer (include/cczero_b200.h): rows of an intermediate buffer of the last forward; synchronises
+int nn_read_buffer(NnRuntime*, int which, int n, void* dst_dev, long long dst_bytes, long long* row_bytes);
 
 }  // namespace cznn

@@ -1133,6 +1133,19 @@ int cz_nn_profile(cz_engine* e, int enable, double* ms, uint64_t* launches, doub
 #endif
 }
 
+int cz_nn_read_buffer(cz_engine* e, int32_t which, int32_t n, void* dst_dev, int64_t dst_bytes, int64_t* row_bytes) {
+#if defined(CZ_EMUL)
+  (void)e; (void)which; (void)n; (void)dst_dev; (void)dst_bytes; (void)row_bytes;
+  return cz_fail(CZ_ERR_UNSUPPORTED, "cz_nn_read_buffer: no network in the CPU emulation build");
+#else
+  if (!e || !e->nn) return cz_fail(CZ_ERR_STATE, "cz_nn_read_buffer: engine has no network");
+  long long rb = 0;
+  const int rc = cznn::nn_read_buffer(e->nn, which, n, dst_dev, (long long)dst_bytes, &rb);
+  if (row_bytes) *row_bytes = rb;
+  return rc;
+#endif
+}
+
 }  // extern "C"
 
 #include "cz_selfplay_api.inc"

@@ -122,6 +122,7 @@ _SIGS = {
     "cz_igemm_conv3x3": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "cz_igemm_conv3x3_dense": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "cz_igemm_dense": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
+    "cz_nn_read_buffer": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
 }
 # entry points that only exist in the CUDA build (tensor cores cannot be emulated on the CPU)
 CUDA_ONLY = {"cz_igemm_conv3x3", "cz_igemm_conv3x3_dense", "cz_igemm_dense"}

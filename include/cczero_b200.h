@@ -325,6 +325,30 @@ int cz_noise_sample(cz_engine* e, int game, int n_moves, int count, double* out_
  * out f32 [m][ldo], 16-byte aligned with ldo a multiple of 4. */
 int cz_igemm_dense(const void* a_dev, const void* w_dev, const float* bias_dev, float* out_dev, int m, int n_valid,
                    int n_pad, int k, int n_tile, int ldo, void* stream);
+/* Intermediate buffers of the network forward, as the last cz_nn_forward / cz_nn_forward_boards left them (dense layout;
+ * rows = positions, C = nn_filters):
+ *   FIRST_OUT    fp16 [90][C]  first convolution + BN + ReLU (1-block nets only: deeper towers overwrite it)
+ *   FIRST_OUT32  f32  [90][C]  its fp32 skip-stream copy (fp32 skip stream and 1 block only)
+ *   LAST_CONV1   fp16 [90][C]  first convolution of the last residual block
+ *   TOWER_OUT    fp16 [90][C]  output of the residual tower (what the heads read)
+ *   TOWER_OUT32  f32  [90][C]  its fp32 skip-stream copy (fp32 skip stream only; the heads read this one then)
+ *   POL_FEAT     fp16 [3 * pol_k1]  policy features split as [hi | lo | hi], pol_k1 = policy channels * 90 padded to 64
+ *   LOGITS       f32  [2304]   policy logits (labels 2086.. are padding)
+ *   STATS        float2 [9]    per 256-label tile {max logit, sum exp(logit - max)} of the policy GEMM epilogue */
+typedef enum cz_nn_buffer {
+  CZ_NN_BUF_FIRST_OUT = 0,
+  CZ_NN_BUF_FIRST_OUT32 = 1,
+  CZ_NN_BUF_LAST_CONV1 = 2,
+  CZ_NN_BUF_TOWER_OUT = 3,
+  CZ_NN_BUF_TOWER_OUT32 = 4,
+  CZ_NN_BUF_POL_FEAT = 5,
+  CZ_NN_BUF_LOGITS = 6,
+  CZ_NN_BUF_STATS = 7
+} cz_nn_buffer;
+/* Copy the first n position rows of buffer `which` (cz_nn_buffer) to dst_dev; *row_bytes = bytes per row.  dst_dev = NULL
+ * only reports row_bytes.  CZ_ERR_ARG: unknown buffer, n > max batch or dst_bytes < n * row_bytes; CZ_ERR_STATE: the
+ * buffer does not exist in this configuration; CZ_ERR_UNSUPPORTED: strip layout (CZ_CONV_STRIP=1).  Synchronises. */
+int cz_nn_read_buffer(cz_engine* e, int32_t which, int32_t n, void* dst_dev, int64_t dst_bytes, int64_t* row_bytes);
 
 #ifdef __cplusplus
 }

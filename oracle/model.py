@@ -83,41 +83,128 @@ def init_weights(filters, blocks, value_fc=256, seed=0, trained_like=False, spre
     return w
 
 
-def _find(w, layer, weight):
+def _array(w, layer, weight):
     for k, v in w.items():
         l, ww = k.split("/", 1)
         if ww.split(":")[0] == weight and (l == layer or l.startswith(layer + "-")):
-            return torch.as_tensor(np.asarray(v), dtype=torch.float32)
+            return np.asarray(v, dtype=np.float32)
     raise KeyError((layer, weight))
 
 
+def _find(w, layer, weight, dtype=torch.float32, device="cpu"):
+    return torch.as_tensor(_array(w, layer, weight), dtype=torch.float32).to(device=device, dtype=dtype)
+
+
 def _conv(x, w, layer, pad):
-    k = _find(w, layer, "kernel").permute(3, 2, 0, 1).contiguous()      # HWIO -> OIHW
+    k = _find(w, layer, "kernel", x.dtype, x.device).permute(3, 2, 0, 1).contiguous()      # HWIO -> OIHW
     return F.conv2d(x, k, padding=pad)
 
 
 def _bn(x, w, layer):
-    g, b = _find(w, layer, "gamma"), _find(w, layer, "beta")
-    m, v = _find(w, layer, "moving_mean"), _find(w, layer, "moving_variance")
+    g, b = _find(w, layer, "gamma", x.dtype, x.device), _find(w, layer, "beta", x.dtype, x.device)
+    m, v = _find(w, layer, "moving_mean", x.dtype, x.device), _find(w, layer, "moving_variance", x.dtype, x.device)
     sh = (1, -1, 1, 1)
     return (x - m.view(sh)) / torch.sqrt(v.view(sh) + BN_EPS) * g.view(sh) + b.view(sh)
 
 
-def forward(w, planes, blocks):
-    """planes: float32 [B,14,10,9] -> (policy [B,2086] softmax, value [B]) in fp32 on the CPU."""
-    x = torch.as_tensor(np.asarray(planes), dtype=torch.float32)
+def forward_stages(w, planes, blocks, dtype=torch.float64, device="cpu"):
+    """The network in `dtype` on `device` (float64 by default: the reference the GPU kernels are measured against), with
+    every stage kept: first [B,C,10,9] (input conv + BN + ReLU), conv1[i] / out[i] (first conv + BN + ReLU / output of
+    residual block i), pol_feat [B, policy channels * 90] (Keras Flatten of channels_first), logits [B,2086], policy
+    (softmax), log_policy (log-softmax in `dtype`), value_pre [B] (before tanh), value [B]."""
+    def dense(x, layer):
+        return x @ _find(w, layer, "kernel", dtype, device) + _find(w, layer, "bias", dtype, device)
+
+    x = torch.as_tensor(np.asarray(planes), dtype=torch.float32).to(device=device, dtype=dtype)
+    st = {"conv1": [], "out": []}
     with torch.no_grad():
         x = F.relu(_bn(_conv(x, w, "input_conv", 2), w, "input_batchnorm"))
+        st["first"] = x
         for i in range(1, blocks + 1):
             y = F.relu(_bn(_conv(x, w, f"res{i}_conv1", 1), w, f"res{i}_batchnorm1"))
+            st["conv1"].append(y)
             y = _bn(_conv(y, w, f"res{i}_conv2", 1), w, f"res{i}_batchnorm2")
             x = F.relu(x + y)
+            st["out"].append(x)
         p = F.relu(_bn(_conv(x, w, "policy_conv", 0), w, "policy_batchnorm")).flatten(1)
-        p = torch.softmax(p @ _find(w, "policy_out", "kernel") + _find(w, "policy_out", "bias"), dim=1)
+        st["pol_feat"] = p
+        st["logits"] = dense(p, "policy_out")
+        st["policy"] = torch.softmax(st["logits"], dim=1)
+        st["log_policy"] = torch.log_softmax(st["logits"], dim=1)
         v = F.relu(_bn(_conv(x, w, "value_conv", 0), w, "value_batchnorm")).flatten(1)
-        v = F.relu(v @ _find(w, "value_dense", "kernel") + _find(w, "value_dense", "bias"))
-        v = torch.tanh(v @ _find(w, "value_out", "kernel") + _find(w, "value_out", "bias"))
-    return p.numpy(), v.numpy()[:, 0]
+        v = F.relu(dense(v, "value_dense"))
+        st["value_pre"] = dense(v, "value_out")[:, 0]
+        st["value"] = torch.tanh(st["value_pre"])
+    return st
+
+
+def forward(w, planes, blocks):
+    """planes: float32 [B,14,10,9] -> (policy [B,2086] softmax, value [B]) in fp32 on the CPU."""
+    st = forward_stages(w, planes, blocks, dtype=torch.float32)
+    return st["policy"].numpy(), st["value"].numpy()
+
+
+def _bn_fold(w, layer):
+    """k_bn_fold in float32: scale = gamma / sqrt(var + eps), shift = beta - mean * scale; also |beta| + |mean * scale|, the
+    magnitude of the shift's terms."""
+    g, b = _array(w, layer, "gamma"), _array(w, layer, "beta")
+    m, v = _array(w, layer, "moving_mean"), _array(w, layer, "moving_variance")
+    s = g / np.sqrt(v + np.float32(BN_EPS))
+    return s, b - m * s, np.abs(b) + np.abs(m * s)
+
+
+def _split16(f):
+    """f32 -> (hi, lo) fp16 with hi = RN(f), lo = RN(f - hi) (f - hi is exact in f32)."""
+    hi = f.astype(np.float16)
+    return hi, (f - hi.astype(np.float32)).astype(np.float16)
+
+
+def folded_operands(w, in_planes=14):
+    """The operands cz_nn.cu's weight preparation builds from a Keras weight dict, restated in float32 numpy:
+      w_first     fp16 [5][5][in_planes][C]  input conv, HWIO, BN scale folded (k_prep_hwio)
+      w_conv[l]   fp16 [9][C_out][C_in]       residual conv l = 2*block + j, tap-major, BN scale folded (k_prep_conv3)
+      wh          f32  [pol_c + val_c][C]     policy then value 1x1 conv, BN scale folded (k_prep_1x1)
+      w_pol       fp16 [2304][3 * pol_k1]     policy Dense split as [w_hi | w_hi | w_lo], zero padded (k_prep_policy)
+      shift_first, shift_conv[l], shifth: BN shifts (f32); b_pol f32 [2304]; wv1, bv1, wv2, bv2: value Dense copies.
+      shift_first_abs, shift_conv_abs[l], shifth_abs: |beta| + |mean * scale|, the magnitude of each shift's terms.
+    Division and sqrt are correctly rounded on both sides, so the fp16 operands agree bit for bit with the GPU's.  A shift
+    may differ where nvcc contracts beta - mean * scale into an FMA: by half an f32 ulp of mean * scale, which exceeds an
+    ulp of the shift itself when the two terms cancel (hence the *_abs magnitudes)."""
+    out = {}
+    s, out["shift_first"], out["shift_first_abs"] = _bn_fold(w, "input_batchnorm")
+    k = _array(w, "input_conv", "kernel")
+    assert k.shape[2] == in_planes, (k.shape, in_planes)
+    out["w_first"] = (k * s).astype(np.float16)
+    blocks = sum(1 for key in w if key.startswith("res") and "_conv1" in key and key.endswith("/kernel"))
+    out["w_conv"], out["shift_conv"], out["shift_conv_abs"] = [], [], []
+    for i in range(1, blocks + 1):
+        for j in (1, 2):
+            s, sh, sha = _bn_fold(w, f"res{i}_batchnorm{j}")
+            k = _array(w, f"res{i}_conv{j}", "kernel")                         # [3][3][ci][co]
+            c = k.shape[3]
+            out["w_conv"].append((k * s).astype(np.float16).reshape(9, c, c).transpose(0, 2, 1).copy())
+            out["shift_conv"].append(sh)
+            out["shift_conv_abs"].append(sha)
+    heads, shifts, shifts_abs = [], [], []
+    for conv, bn in (("policy_conv", "policy_batchnorm"), ("value_conv", "value_batchnorm")):
+        s, sh, sha = _bn_fold(w, bn)
+        heads.append((_array(w, conv, "kernel")[0, 0] * s).T)                 # [ci][co] -> [co][ci]
+        shifts.append(sh)
+        shifts_abs.append(sha)
+    out["pol_c"], out["val_c"] = heads[0].shape[0], heads[1].shape[0]
+    out["wh"], out["shifth"], out["shifth_abs"] = np.concatenate(heads), np.concatenate(shifts), np.concatenate(shifts_abs)
+    pol_in = 90 * out["pol_c"]
+    pol_k1 = (pol_in + 63) // 64 * 64
+    f = np.zeros((2304, pol_k1), np.float32)
+    f[:N_LABELS, :pol_in] = _array(w, "policy_out", "kernel").T
+    hi, lo = _split16(f)
+    out["pol_k1"], out["w_pol"] = pol_k1, np.concatenate([hi, hi, lo], axis=1)
+    out["b_pol"] = np.zeros(2304, np.float32)
+    out["b_pol"][:N_LABELS] = _array(w, "policy_out", "bias")
+    for name, layer, weight in (("wv1", "value_dense", "kernel"), ("bv1", "value_dense", "bias"),
+                                ("wv2", "value_out", "kernel"), ("bv2", "value_out", "bias")):
+        out[name] = _array(w, layer, weight)
+    return out
 
 
 class TorchNet:
