@@ -22,7 +22,7 @@ EMUL_LIB = os.path.join(ROOT, "tests", "simt_emul", "libcz_emul.so")
 #   integer / tree code is compiled with -fmad=false so that fp64 PUCT arithmetic rounds exactly
 #   like the reference's Python floats (no contraction of a*b+c into fma).
 INT_UNITS = ["cz_env_api.cu", "cz_tree_api.cu"]
-NN_UNITS = ["cz_nn.cu"]
+NN_UNITS = ["cz_nn.cu", "cz_train.cu"]
 HOST_UNITS = ["cz_err.cpp"]
 
 NVCC_COMMON = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

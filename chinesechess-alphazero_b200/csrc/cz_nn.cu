@@ -22,6 +22,7 @@
 #include "cz_err.h"
 #include "cz_igemm.cuh"
 #include "cz_nn.cuh"
+#include "cz_nn_host.cuh"
 
 namespace cznn {
 
@@ -67,16 +68,17 @@ static int load_encode() {
 }
 
 // fp16 NHWC activations [n][10][9][c] read in im2col mode for a 3x3 "same" convolution: the bounding box of base pixels is
-// [-1, dim-2] in w and h (lower corner = -pad, upper corner = pad - (filter-1)), 64 channels x 128 output pixels per load;
-// taps outside the image are zero-filled by the TMA unit, and the 128-pixel column walks across rows and images.
-static int make_map_im2col(CUtensorMap* m, const void* base, int c, long long n_images) {
+// [-1, dim-2] in w and h (lower corner = -pad, upper corner = pad - (filter-1)), 64 channels x `pixels` (128 for the forward)
+// output pixels per load;
+// taps outside the image are zero-filled by the TMA unit, and the pixel column walks across rows and images.
+int make_map_im2col(CUtensorMap* m, const void* base, int c, long long n_images, int pixels) {
   if (load_encode()) return CZ_ERR_CUDA;
   if (!g_encode_im2col) return cz_fail(CZ_ERR_UNSUPPORTED, "cuTensorMapEncodeIm2col not available");
   cuuint64_t dims[4] = {(cuuint64_t)c, 9, 10, (cuuint64_t)n_images};
   cuuint64_t strides[3] = {(cuuint64_t)c * 2, (cuuint64_t)c * 2 * 9, (cuuint64_t)c * 2 * 90};
   int lower[2] = {-1, -1}, upper[2] = {-1, -1};
   cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = g_encode_im2col(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, lower, upper, 64, 128,
+  CUresult r = g_encode_im2col(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, lower, upper, 64, (cuuint32_t)pixels,
                                es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return cz_fail(CZ_ERR_CUDA, "cuTensorMapEncodeIm2col failed: %d", (int)r);
@@ -97,7 +99,7 @@ static int make_map_3d(CUtensorMap* m, const void* base, int c, int w, long long
   return 0;
 }
 // fp16 matrix [rows][k] (k contiguous), box {64, box_rows}
-static int make_map_2d(CUtensorMap* m, const void* base, int k, long long rows, int box_rows) {
+int make_map_2d(CUtensorMap* m, const void* base, int k, long long rows, int box_rows) {
   if (load_encode()) return CZ_ERR_CUDA;
   cuuint64_t dims[2] = {(cuuint64_t)k, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)k * 2};
@@ -111,7 +113,7 @@ static int make_map_2d(CUtensorMap* m, const void* base, int k, long long rows, 
 }
 
 static int g_num_sms = 0;
-static int num_sms() {
+int num_sms() {
   if (!g_num_sms) {
     int dev = 0;
     cudaGetDevice(&dev);
@@ -155,7 +157,7 @@ static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const 
   CZ_CUDA(cudaGetLastError());
   return 0;
 }
-static int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, const igemm::Args& a, cudaStream_t st) {
+int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, const igemm::Args& a, cudaStream_t st) {
   switch (n_tile) {
     case 64: return launch_igemm_t<64>(tmA, tmB, a, st);
     case 128: return launch_igemm_t<128>(tmA, tmB, a, st);

@@ -139,4 +139,33 @@ struct Wgmma<256> {
   }
 };
 
+// MN-major operand tile (the M / N index contiguous): 128-byte rows of 64 fp16 along M / N, one row per k, SWIZZLE_128B:
+// 8 k-rows form a 1024 B atom.  SBO = 1024 B steps from one 8-k group to the next; LBO steps between 64-wide M / N atoms,
+// which a 64-wide operand never takes, so it is set to the same 1024 B.  A k16 step advances the start address by 2048 B.
+__device__ __forceinline__ uint64_t smem_desc_sw128_mn(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
+  d |= (uint64_t)(1024 >> 4) << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
+
+// D[64 x N] (+)= A[64 x 16] * B[16 x N] with BOTH operands MN-major in smem (tnspA = tnspB = 1); same accumulator layout as Wgmma.
+template <int N>
+struct WgmmaT;
+template <>
+struct WgmmaT<64> {
+  __device__ __forceinline__ static void mma(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate));
+  }
+};
+
 }  // namespace wg

@@ -69,6 +69,17 @@ class CzTensorDesc(C.Structure):
     _fields_ = [("name", C.c_char_p), ("dev", C.c_void_p), ("numel", C.c_int64)]
 
 
+class CzTrainConfig(C.Structure):
+    _fields_ = [("struct_bytes", C.c_int32), ("filters", C.c_int32), ("blocks", C.c_int32), ("in_planes", C.c_int32),
+                ("policy_channels", C.c_int32), ("value_channels", C.c_int32), ("value_fc", C.c_int32),
+                ("max_batch", C.c_int32)]
+
+
+class CzTrainHparams(C.Structure):
+    _fields_ = [("struct_bytes", C.c_int32), ("lr", C.c_float), ("momentum", C.c_float), ("w_policy", C.c_float),
+                ("w_value", C.c_float), ("l2", C.c_float)]
+
+
 _P = C.c_void_p
 _SIGS = {
     "cz_last_error": (C.c_char_p, []),
@@ -123,9 +134,20 @@ _SIGS = {
     "cz_igemm_conv3x3_dense": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "cz_igemm_dense": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "cz_nn_read_buffer": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
+    "cz_train_workspace_bytes": (C.c_int, [C.POINTER(CzTrainConfig), C.POINTER(C.c_uint64)]),
+    "cz_train_create": (C.c_int, [C.POINTER(CzTrainConfig), _P, C.c_uint64, _P, C.POINTER(_P)]),
+    "cz_train_destroy": (None, [_P]),
+    "cz_train_set_params": (C.c_int, [_P, C.POINTER(CzTensorDesc), C.c_int32, C.POINTER(CzTensorDesc), C.c_int32]),
+    "cz_train_step": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.POINTER(CzTrainHparams), _P]),
+    "cz_train_read_grad": (C.c_int, [_P, C.c_char_p, _P, C.c_int64]),
+    "cz_train_wgrad3x3": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
+    "cz_train_dgrad3x3": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P]),
+    "cz_train_bn": (C.c_int, [_P, C.c_longlong, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
 }
 # entry points that only exist in the CUDA build (tensor cores cannot be emulated on the CPU)
-CUDA_ONLY = {"cz_igemm_conv3x3", "cz_igemm_conv3x3_dense", "cz_igemm_dense"}
+CUDA_ONLY = {"cz_igemm_conv3x3", "cz_igemm_conv3x3_dense", "cz_igemm_dense", "cz_train_workspace_bytes", "cz_train_create",
+             "cz_train_destroy", "cz_train_set_params", "cz_train_step", "cz_train_read_grad", "cz_train_wgrad3x3",
+             "cz_train_dgrad3x3", "cz_train_bn"}
 
 
 class CzLib:

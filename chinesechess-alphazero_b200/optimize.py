@@ -1,0 +1,239 @@
+"""`worker.optimize` drop-in (reference: cchess_alphazero/worker/optimize.py:37-225): learn from the play-data files.
+
+`start(config)` and `OptimizeWorker(config)` keep the reference's method names and control flow: take the play-data
+files in batches of `load_step` (`load_data_steps` where the config has no `load_step`), expand them into training
+tensors (`records.expanding_data`, on the rules kernels), run `epoch_to_checkpoint` epochs of Keras-`fit`-equivalent
+training, save the best model, move the used files to `data/trained/`, and when the files run out save the next
+generation.  The reference compiles a Keras model and calls `fit`; here `compile_model` builds a `train.Trainer`
+(cz_train_step: CUDA forward, backward and SGD-momentum update) and `fit` restates Keras 2.0.8's loop: the last 2 % of
+the samples (before shuffling) validate, the training indices are reshuffled every epoch with numpy's global RNG, the
+final partial batch is kept, lr is constant within one call, and the validation loss is computed in inference mode.
+"""
+import os
+import shutil
+from collections import deque
+from logging import getLogger
+from random import shuffle
+from types import SimpleNamespace
+
+import numpy as np
+
+from .model import CChessModel
+from .records import expanding_data, get_game_data_filenames, read_game_data_from_file
+
+logger = getLogger(__name__)
+
+
+def start(config):
+    return OptimizeWorker(config).start()
+
+
+def load_best_model_weight(model):
+    rc = model.config.resource
+    return model.load(rc.model_best_config_path, rc.model_best_weight_path)
+
+
+def save_as_best_model(model):
+    rc = model.config.resource
+    model.save(rc.model_best_config_path, rc.model_best_weight_path)
+
+
+def save_as_next_generation_model(model):
+    rc = model.config.resource
+    model.save(rc.next_generation_config_path, rc.next_generation_weight_path)
+
+
+def load_data_from_file(filename, env, use_history=False):
+    """optimize.py:223-232: a file that cannot be read is deleted.  Where the reference's expanding_data reads a file as ONE
+    game (and rejects files of several games: the second initial state is not a move), every game of the file is expanded."""
+    try:
+        data = read_game_data_from_file(filename)
+    except Exception as e:
+        logger.error(f"Error when loading data {e}")
+        os.remove(filename)
+        return None
+    if data is None:
+        return None
+    games = [[]]
+    for item in data:                     # a file holds nb_game_in_file games back to back: [state, moves..., state, moves...]
+        if isinstance(item, str) and games[-1]:
+            games.append([])
+        games[-1].append(item)
+    out = [expanding_data(g, env, use_history) for g in games if len(g) > 1]
+    if not out:
+        return None
+    return tuple(np.concatenate([o[i] for o in out]) for i in range(3))
+
+
+def validation_split(n, split=0.02):
+    """Keras 2.0.8 fit(validation_split=...): split_at = int(n * (1 - split)), the last samples validate."""
+    split_at = int(n * (1.0 - split))
+    return np.arange(split_at), np.arange(split_at, n)
+
+
+def make_batches(size, batch_size):
+    """Keras _make_batches: ceil(size / batch_size) slices, the last one partial."""
+    nb = int(np.ceil(size / float(batch_size)))
+    return [(i * batch_size, min(size, (i + 1) * batch_size)) for i in range(nb)]
+
+
+class OptimizeWorker:
+    def __init__(self, config, env=None, trainer_factory=None, device=None):
+        """env: StaticEnv for expanding records (default: the CUDA rules kernels); trainer_factory(model, batch_size, device)
+        builds the object whose step(planes, policy, value, lr) / validation_loss(...) / export() train (default
+        train.Trainer)."""
+        self.config = config
+        self.model = None
+        self.loaded_filenames = set()
+        self.loaded_data = deque(maxlen=self.config.trainer.dataset_size)
+        self.dataset = deque(), deque(), deque()
+        self.filenames = []
+        self.opt = None
+        self.count = 0
+        self.eva = False
+        self.env = env
+        self.trainer_factory = trainer_factory
+        self.device = device
+        self.trainer = None
+        self.history = []
+
+    def start(self):
+        self.model = self.load_model()
+        self.training()
+
+    def _env(self):
+        if self.env is None:
+            from .env import StaticEnv
+            from .lib import get_lib
+            self.env = StaticEnv(get_lib(), self.device or "cuda")
+        return self.env
+
+    def training(self):
+        """optimize.py:56-100."""
+        self.compile_model()
+        tc = self.config.trainer
+        total_steps = tc.start_total_steps
+        last_file = None
+        load_step = getattr(tc, "load_step", None) or tc.load_data_steps
+        while True:
+            files = get_game_data_filenames(self.config.resource)
+            offset = tc.min_games_to_begin_learn
+            if (len(files) < tc.min_games_to_begin_learn
+                    or ((last_file is not None and last_file in files) and files.index(last_file) + 1 + offset > len(files))):
+                if last_file is not None:
+                    self.save_current_model(send=True)
+                break
+            if last_file is not None and last_file in files:
+                idx = files.index(last_file) + 1
+                files = files[idx:idx + load_step] if len(files) - idx > load_step else files[idx:]
+            elif len(files) > load_step:
+                files = files[0:load_step]
+            last_file = files[-1]
+            logger.info(f"Last file = {last_file}")
+            self.filenames = deque(files)
+            shuffle(self.filenames)
+            self.fill_queue()
+            self.update_learning_rate(total_steps)
+            if len(self.dataset[0]) > tc.batch_size:
+                steps = self.train_epoch(tc.epoch_to_checkpoint)
+                total_steps += steps
+                self.save_current_model(send=False)
+                self.update_learning_rate(total_steps)
+                self.count += 1
+                self.dataset = deque(), deque(), deque()
+                self.backup_play_data(files)
+        return total_steps
+
+    def train_epoch(self, epochs):
+        """optimize.py:102-121."""
+        tc = self.config.trainer
+        state_ary, policy_ary, value_ary = self.collect_all_loaded_data()
+        self.fit(state_ary, policy_ary, value_ary, tc.batch_size, epochs)
+        return (state_ary.shape[0] // tc.batch_size) * epochs
+
+    def fit(self, x, policy, value, batch_size, epochs, validation=0.02):
+        """Model.fit(x, [policy, value], batch_size, epochs, shuffle=True, validation_split=0.02) of Keras 2.0.8."""
+        train_idx, val_idx = validation_split(len(x), validation)
+        lr = self.opt.lr
+        for epoch in range(epochs):
+            order = train_idx.copy()
+            np.random.shuffle(order)
+            losses = []
+            for a, b in make_batches(len(order), batch_size):
+                ids = order[a:b]
+                losses.append(self.trainer.step(x[ids], policy[ids], value[ids], lr))
+            rec = {"epoch": epoch, "lr": lr, "loss": float(np.mean([l[0] for l in losses])) if losses else None}
+            if len(val_idx):
+                rec["val_loss"] = self.trainer.validation_loss(x[val_idx], policy[val_idx], value[val_idx])[0]
+            logger.info(f"epoch {epoch + 1}/{epochs}: {rec}")
+            self.history.append(rec)
+
+    def compile_model(self):
+        """optimize.py:129-136: SGD(lr=0.02, momentum) on the two losses with config.trainer.loss_weights."""
+        self.opt = SimpleNamespace(lr=0.02, momentum=self.config.trainer.momentum)
+        if self.trainer_factory is not None:
+            self.trainer = self.trainer_factory(self.model, self.config.trainer.batch_size, self.device)
+        else:
+            from .train import Trainer
+            self.trainer = Trainer(self.model, self.config.trainer.batch_size, self.device)
+
+    def update_learning_rate(self, total_steps):
+        lr = self.decide_learning_rate(total_steps)
+        if lr:
+            self.opt.lr = lr
+            logger.debug(f"total step={total_steps}, set learning rate to {lr}")
+
+    def fill_queue(self):
+        """optimize.py:150-170, sequential: files popped from the end of the shuffled list until dataset_size samples."""
+        use_history = bool(getattr(getattr(self.config, "opts", None), "has_history", False))
+        while self.filenames and len(self.dataset[0]) < self.config.trainer.dataset_size:
+            t = load_data_from_file(self.filenames.pop(), self._env(), use_history)
+            if t is not None:
+                for x, y in zip(self.dataset, t):
+                    x.extend(y)
+
+    def collect_all_loaded_data(self):
+        state_ary, policy_ary, value_ary = self.dataset
+        return (np.asarray(state_ary, dtype=np.float32), np.asarray(policy_ary, dtype=np.float32),
+                np.asarray(value_ary, dtype=np.float32))
+
+    def load_model(self):
+        model = CChessModel(self.config)
+        if getattr(getattr(self.config, "opts", None), "new", False) or not load_best_model_weight(model):
+            model.build()
+            save_as_best_model(model)
+        return model
+
+    def save_current_model(self, send=False):
+        logger.info("Save as ng model")
+        if self.trainer is not None:
+            self.model.weights = self.trainer.export()
+        if not send:
+            save_as_best_model(self.model)
+        else:
+            save_as_next_generation_model(self.model)
+
+    def decide_learning_rate(self, total_steps):
+        ret = None
+        for step, lr in self.config.trainer.lr_schedules:
+            if total_steps >= step:
+                ret = lr
+        return ret
+
+    def try_reload_model(self):
+        digest = self.model.fetch_digest(self.config.resource.model_best_weight_path)
+        if digest and digest != self.model.digest:
+            load_best_model_weight(self.model)
+            return True
+        return False
+
+    def backup_play_data(self, files):
+        backup_folder = os.path.join(self.config.resource.data_dir, "trained")
+        cnt = 0
+        os.makedirs(backup_folder, exist_ok=True)
+        for f in files:
+            try:
+                shutil.move(f, backup_folder)
+            except Exception:
+                cnt += 1
+        logger.info(f"backup {len(files)} files, {cnt} empty files")

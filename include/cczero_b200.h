@@ -350,6 +350,55 @@ typedef enum cz_nn_buffer {
  * buffer does not exist in this configuration; CZ_ERR_UNSUPPORTED: strip layout (CZ_CONV_STRIP=1).  Synchronises. */
 int cz_nn_read_buffer(cz_engine* e, int32_t which, int32_t n, void* dst_dev, int64_t dst_bytes, int64_t* row_bytes);
 
+/* ------------------------------------------------------------------------------------------
+ * Training — one Keras Model.fit batch of worker/optimize.py:108-136 (SGD momentum, categorical cross-entropy + MSE
+ * + L2, BatchNormalization in training mode).  Same conventions as the engine: one caller-owned device workspace
+ * (cz_train_workspace_bytes), caller-owned device tensors passed by pointer, stream-ordered calls, a negative cz_status
+ * with a message in cz_last_error() on error.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct cz_trainer cz_trainer;
+typedef struct cz_train_config {
+  int32_t struct_bytes;        /* sizeof(cz_train_config) */
+  int32_t filters;             /* cnn_filter_num: 64..256, multiple of 64 */
+  int32_t blocks;              /* res_layer_num */
+  int32_t in_planes;           /* 14, or 28 with use_history */
+  int32_t policy_channels;     /* 1x1 policy conv filters (agent/model.py: 4; legacy configs 2 or 32) */
+  int32_t value_channels;      /* 1x1 value conv filters (2; legacy 4) */
+  int32_t value_fc;            /* value_fc_size, <= 256 */
+  int32_t max_batch;           /* largest batch of cz_train_step, <= 4096 */
+} cz_train_config;
+typedef struct cz_train_hparams {
+  int32_t struct_bytes;        /* sizeof(cz_train_hparams) */
+  float lr, momentum;          /* SGD: v = momentum * v - lr * g; w += v */
+  float w_policy, w_value;     /* config.trainer.loss_weights */
+  float l2;                    /* config.model.l2_reg: loss += l2 * sum K^2 over conv and Dense kernels */
+} cz_train_hparams;
+int cz_train_workspace_bytes(const cz_train_config* cfg, uint64_t* bytes);
+int cz_train_create(const cz_train_config* cfg, void* workspace_dev, uint64_t bytes, void* stream, cz_trainer** out);
+void cz_train_destroy(cz_trainer* t);
+/* params: every weight in Keras names and layouts (f32, including BN moving_mean / moving_variance); velocity: one
+ * tensor per trainable weight (kernels, biases, BN gamma / beta), same names and sizes.  cz_train_step updates both IN
+ * PLACE (and the moving statistics).  CZ_ERR_ARG: a tensor is missing or has the wrong size. */
+int cz_train_set_params(cz_trainer* t, const cz_tensor_desc* params, int32_t n, const cz_tensor_desc* velocity, int32_t n_velocity);
+/* One step on `batch` samples: planes_dev [B][in_planes][10][9] f32 (one-hot), policy_target_dev [B][2086] f32,
+ * value_target_dev [B] f32.  losses_dev[4] f32 = {total, policy cross-entropy, value MSE, l2 term} before the update.
+ * CZ_ERR_ARG: batch outside 1..max_batch; CZ_ERR_STATE: no parameters set.  Bit-reproducible. */
+int cz_train_step(cz_trainer* t, const float* planes_dev, const float* policy_target_dev, const float* value_target_dev,
+                  int32_t batch, const cz_train_hparams* hp, float* losses_dev);
+/* Tests: copy the last step's gradient of one trainable weight (loss terms only, without the L2 part).  CZ_ERR_ARG:
+ * unknown name or numel differs.  Synchronises; off the step path. */
+int cz_train_read_grad(cz_trainer* t, const char* name, void* dst_dev, int64_t numel);
+/* Stage building blocks of the step, for parity tests (allocate scratch, synchronise):
+ *   wgrad3x3  dw (Keras HWIO [3][3][c][c] f32) of a 3x3 "same" conv: x16 fp16 [n][10][9][c], dy f32 [n*90][c]
+ *   dgrad3x3  dx f32 [n*90][c] = input gradient of that conv for HWIO weights w_hwio f32
+ *   bn        training-mode BN (+ skip) + ReLU on z [rows][c]: out, batch mean, biased var; with up (gradient of the
+ *             ReLU output) also dz, dgamma, dbeta */
+int cz_train_wgrad3x3(const void* x16_dev, const float* dy_dev, int n, int c, float* dw_dev, void* stream);
+int cz_train_dgrad3x3(const float* dy_dev, const float* w_hwio_dev, int n, int c, float* dx_dev, void* stream);
+int cz_train_bn(const float* z_dev, long long rows, int c, const float* gamma_dev, const float* beta_dev, const float* skip_dev,
+                float* out_dev, float* mean_dev, float* var_dev, const float* up_dev, float* dz_dev, float* dgamma_dev,
+                float* dbeta_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
