@@ -21,7 +21,7 @@ EMUL_LIB = os.path.join(ROOT, "tests", "simt_emul", "libcz_emul.so")
 # translation units: (file, extra nvcc flags)
 #   integer / tree code is compiled with -fmad=false so that fp64 PUCT arithmetic rounds exactly
 #   like the reference's Python floats (no contraction of a*b+c into fma).
-INT_UNITS = ["cz_env_api.cu", "cz_tree_api.cu"]
+INT_UNITS = ["cz_env_api.cu", "cz_tree_api.cu", "cz_replay.cu"]
 NN_UNITS = ["cz_nn.cu", "cz_train.cu"]
 HOST_UNITS = ["cz_err.cpp"]
 

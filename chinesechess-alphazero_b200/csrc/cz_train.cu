@@ -423,6 +423,31 @@ __global__ void k_sgd(float* __restrict__ w, float* __restrict__ v, const float*
     w[i] += vn;
   }
 }
+// Keras 2.0.8 Adam (decay 0), every trainable tensor in ONE launch: block b updates chunk b - block0 of the segment that
+// owns it.  The operations are spelled out (no contraction) so that a float32 restatement in the same order is bit-exact:
+//   g = grad + 2*l2*w (kernels);  m = b1*m + (1-b1)*g;  v = b2*v + (1-b2)*g*g;  w = w - (lr_t*m) / (sqrt(v) + eps)
+constexpr int kAdamChunk = 2048;
+struct AdamSeg { float* w; float* m; float* v; const float* g; long long n; long long block0; int reg; int pad; };
+__global__ void k_adam(const AdamSeg* __restrict__ seg, int nseg, float lr_t, float b1, float omb1, float b2, float omb2, float eps,
+                       float l2x2) {
+  int lo = 0, hi = nseg - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (seg[mid].block0 <= (long long)blockIdx.x) lo = mid; else hi = mid - 1;
+  }
+  const AdamSeg s = seg[lo];
+  const long long base = ((long long)blockIdx.x - s.block0) * kAdamChunk;
+  const long long end = base + kAdamChunk < s.n ? base + kAdamChunk : s.n;
+  for (long long i = base + threadIdx.x; i < end; i += blockDim.x) {
+    const float w = s.w[i];
+    const float g = s.reg ? __fadd_rn(s.g[i], __fmul_rn(l2x2, w)) : s.g[i];
+    const float m = __fadd_rn(__fmul_rn(b1, s.m[i]), __fmul_rn(omb1, g));
+    const float v = __fadd_rn(__fmul_rn(b2, s.v[i]), __fmul_rn(omb2, __fmul_rn(g, g)));
+    s.m[i] = m;
+    s.v[i] = v;
+    s.w[i] = __fsub_rn(w, __fdiv_rn(__fmul_rn(lr_t, m), __fadd_rn(__fsqrt_rn(v), eps)));
+  }
+}
 // Keras moving_average_update (TF assign_moving_average, zero_debias off): m -= (m - batch) * (1 - 0.99)
 __global__ void k_moving(float* __restrict__ m, const float* __restrict__ batch, int c) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -448,6 +473,7 @@ struct Param {
   long long numel;
   bool train, reg;             // updated by SGD / carries the L2 penalty (kernels)
   float *w, *v, *g;            // master (caller), velocity (caller), gradient (workspace)
+  float *am, *av;              // Adam moments (caller), set by cz_train_set_adam
 };
 struct Bn {
   int C; int gamma, beta, mm, mv;   // Param indices
@@ -490,6 +516,12 @@ struct Trainer {
   float* scale_slots;                // [2L + 1][4]
   float *Fp, *Fv, *logits, *dlog, *hpre, *hact, *vpre, *dvpre, *dh, *dF, *ce_rows, *se_rows, *ones;
   float* l2_slots; int n_reg;
+  // Adam (cz_train_set_adam): the segment table lives in the workspace
+  bool adam;
+  double b1, b2, eps;
+  long long iterations;
+  AdamSeg* adam_tab; int n_adam; long long adam_blocks;
+  std::vector<AdamSeg> adam_host;
 };
 
 static size_t act_bytes(const Trainer* t, int elem) { return (size_t)t->maxb * 90 * t->C * elem; }
@@ -531,6 +563,7 @@ static void layout(Trainer* t, Carver& cv) {
   t->ones = (float*)cv.take((size_t)B * 4);
   t->l2_slots = (float*)cv.take((size_t)(t->p.size() + 1) * 4);
   for (Param& q : t->p) q.g = (float*)cv.take((size_t)q.numel * 4);
+  t->adam_tab = (AdamSeg*)cv.take(t->p.size() * sizeof(AdamSeg));
 }
 
 static void add_bn(Trainer* t, const std::string& layer, int c) {
@@ -806,8 +839,17 @@ static int step(Trainer* t, const float* planes, const float* pol_t, const float
     if (q.reg) k_sumsq<<<1, 256, 0, st>>>(q.w, q.numel, t->l2_slots + slot++);
   k_losses<<<1, 256, 0, st>>>(t->ce_rows, t->se_rows, n, t->l2_slots, slot, hp.l2, hp.w_policy, hp.w_value, losses);
   // ---------------------------------------------------------------- update
-  for (const Param& q : t->p)
-    if (q.train) k_sgd<<<blocks_for(q.numel), 256, 0, st>>>(q.w, q.v, q.g, q.numel, hp.lr, hp.momentum, q.reg ? 2.f * hp.l2 : 0.f);
+  if (t->adam) {
+    // lr_t = lr * (sqrt(1 - b2^t) / (1 - b1^t)), t = iterations + 1: float64 on the host, rounded to fp32 once
+    const double it = (double)(t->iterations + 1);
+    const float lr_t = (float)((double)hp.lr * (sqrt(1.0 - pow(t->b2, it)) / (1.0 - pow(t->b1, it))));
+    const float b1 = (float)t->b1, b2 = (float)t->b2;
+    k_adam<<<(unsigned)t->adam_blocks, 256, 0, st>>>(t->adam_tab, t->n_adam, lr_t, b1, 1.f - b1, b2, 1.f - b2, (float)t->eps,
+                                                      2.f * hp.l2);
+  } else {
+    for (const Param& q : t->p)
+      if (q.train) k_sgd<<<blocks_for(q.numel), 256, 0, st>>>(q.w, q.v, q.g, q.numel, hp.lr, hp.momentum, q.reg ? 2.f * hp.l2 : 0.f);
+  }
   for (const Bn& b : t->bn) {
     k_moving<<<(b.C + 255) / 256, 256, 0, st>>>(t->p[b.mm].w, b.mean, b.C);
     k_moving<<<(b.C + 255) / 256, 256, 0, st>>>(t->p[b.mv].w, b.var, b.C);
@@ -846,6 +888,7 @@ int cz_train_create(const cz_train_config* cfg, void* workspace, uint64_t bytes,
   init_geometry(t, cfg);
   t->st = (cudaStream_t)stream;
   t->params_set = false; t->last_batch = -1;
+  t->adam = false; t->iterations = 0; t->n_adam = 0; t->adam_blocks = 0;
   Carver cv{(uint8_t*)workspace, 0};
   layout(t, cv);
   const int C = t->C;
@@ -890,6 +933,7 @@ int cz_train_set_params(cz_trainer* h, const cz_tensor_desc* params, int32_t n, 
   }
   for (size_t i = 0; i < t->p.size(); ++i) { t->p[i].w = w[i]; t->p[i].v = v[i]; }
   t->params_set = true;
+  t->adam = false;                   // the Adam table points at the previous weights: register it again
   return 0;
 }
 
@@ -901,7 +945,50 @@ int cz_train_step(cz_trainer* h, const float* planes, const float* policy_target
   if (batch < 1 || batch > t->maxb) return cz_fail(CZ_ERR_ARG, "cz_train_step: batch %d outside 1..%d", batch, t->maxb);
   if (!planes || !policy_target || !value_target || !hp || !losses) return cz_fail(CZ_ERR_ARG, "cz_train_step: null pointer");
   if (hp->struct_bytes != (int)sizeof(cz_train_hparams)) return cz_fail(CZ_ERR_ARG, "cz_train_step: hparams struct_bytes mismatch");
-  return step(t, planes, policy_target, value_target, batch, *hp, losses);
+  const int rc = step(t, planes, policy_target, value_target, batch, *hp, losses);
+  if (!rc && t->adam) ++t->iterations;
+  return rc;
+}
+
+int cz_train_set_adam(cz_trainer* h, const cz_tensor_desc* m, int32_t nm, const cz_tensor_desc* v, int32_t nv, double beta_1,
+                      double beta_2, double epsilon) {
+  if (!h) return cz_fail(CZ_ERR_ARG, "cz_train_set_adam: null trainer");
+  Trainer* t = &h->t;
+  if (!t->params_set) return cz_fail(CZ_ERR_STATE, "cz_train_set_adam: parameters not set (cz_train_set_params)");
+  if (!m || nm <= 0 || !v || nv <= 0) return cz_fail(CZ_ERR_ARG, "cz_train_set_adam: empty tensor list");
+  if (!(beta_1 >= 0.0 && beta_1 < 1.0) || !(beta_2 >= 0.0 && beta_2 < 1.0) || !(epsilon >= 0.0))
+    return cz_fail(CZ_ERR_ARG, "cz_train_set_adam: beta_1, beta_2 must lie in [0, 1) and epsilon >= 0");
+  std::vector<AdamSeg> segs;
+  std::vector<float*> am(t->p.size(), nullptr), av(t->p.size(), nullptr);
+  long long blocks = 0;
+  for (size_t i = 0; i < t->p.size(); ++i) {
+    const Param& q = t->p[i];
+    if (!q.train) continue;
+    const cz_tensor_desc* dm = find_desc(m, nm, q);
+    const cz_tensor_desc* dv = find_desc(v, nv, q);
+    if (!dm || !dm->dev || dm->numel != q.numel || !dv || !dv->dev || dv->numel != q.numel)
+      return cz_fail(CZ_ERR_ARG, "cz_train_set_adam: missing or mis-sized moment %s/%s (want %lld)", q.layer.c_str(), q.weight.c_str(), q.numel);
+    am[i] = (float*)dm->dev; av[i] = (float*)dv->dev;
+    segs.push_back(AdamSeg{q.w, am[i], av[i], q.g, q.numel, blocks, q.reg ? 1 : 0, 0});
+    blocks += (q.numel + kAdamChunk - 1) / kAdamChunk;
+  }
+  if (blocks > 0x7fffffffLL) return cz_fail(CZ_ERR_UNSUPPORTED, "cz_train_set_adam: %lld update blocks", blocks);
+  t->adam_host = segs;
+  CZ_CUDA(cudaMemcpyAsync(t->adam_tab, t->adam_host.data(), segs.size() * sizeof(AdamSeg), cudaMemcpyHostToDevice, t->st));
+  CZ_CUDA(cudaStreamSynchronize(t->st));
+  for (size_t i = 0; i < t->p.size(); ++i) { t->p[i].am = am[i]; t->p[i].av = av[i]; }
+  t->n_adam = (int)segs.size(); t->adam_blocks = blocks;
+  t->b1 = beta_1; t->b2 = beta_2; t->eps = epsilon;
+  t->iterations = 0;
+  t->adam = true;
+  return 0;
+}
+
+int cz_train_adam_iterations(cz_trainer* h, int64_t* out) {
+  if (!h || !out) return cz_fail(CZ_ERR_ARG, "cz_train_adam_iterations: null argument");
+  if (!h->t.adam) return cz_fail(CZ_ERR_STATE, "cz_train_adam_iterations: the trainer does not use Adam");
+  *out = h->t.iterations;
+  return 0;
 }
 
 int cz_train_read_grad(cz_trainer* h, const char* name, void* dst, int64_t numel) {

@@ -1,9 +1,10 @@
 """Training step of the policy-value network on the GPU: what Keras `Model.fit` runs per batch for worker/optimize.py.
 
-`Trainer(model, batch_size, device)` owns the fp32 master weights, the SGD velocity and the trainer workspace as torch
-tensors; `step()` runs one batch through `cz_train_step` (csrc/cz_train.cu: training-mode forward, backward and the
-SGD-momentum update, all CUDA).  `validation_loss()` evaluates with the inference forward of the engine (`cz_nn_forward`,
-BatchNormalization on the moving statistics) — the same network self-play serves.  `export()` hands the weights back in
+`Trainer(model, batch_size, device, optimizer="sgd"|"adam")` owns the fp32 master weights, the SGD velocity (and, for Adam,
+the moments m / v) and the trainer workspace as torch tensors; `step()` runs one batch through `cz_train_step`
+(csrc/cz_train.cu: training-mode forward, backward and the SGD-momentum or fused Keras Adam update, all CUDA).
+`validation_loss()` evaluates with the inference forward of the engine (`cz_nn_forward`, BatchNormalization on the
+moving statistics) — the same network self-play serves.  `export()` hands the weights back in
 Keras names for `CChessModel.save()`.
 """
 import ctypes as C
@@ -37,7 +38,12 @@ def keras_policy_loss(policy, target):
 
 
 class Trainer:
-    def __init__(self, model, batch_size, device=None, lib=None):
+    def __init__(self, model, batch_size, device=None, lib=None, optimizer="sgd", beta_1=0.9, beta_2=0.999, epsilon=1e-8):
+        """optimizer "sgd": Keras SGD with momentum (worker/optimize.py); "adam": Keras 2.0.8 Adam (worker/sl.py), whose
+        moments m / v this object owns and whose `iterations` run on across every step of this trainer."""
+        if optimizer not in ("sgd", "adam"):
+            raise ValueError(f"optimizer must be 'sgd' or 'adam', not {optimizer!r}")
+        self.optimizer = optimizer
         self.model = model
         self.config = model.config
         self.lib = lib or get_lib()
@@ -65,6 +71,13 @@ class Trainer:
         self.lib.call("cz_train_create", C.byref(cfg), C.c_void_p(self.workspace.data_ptr()), nbytes, stream, C.byref(self._h))
         self._pd, self._vd = _descs(self.weights), _descs(self.velocity)
         self.lib.call("cz_train_set_params", self._h, self._pd, len(self.weights), self._vd, len(self.velocity))
+        self.adam_m = self.adam_v = None
+        if optimizer == "adam":
+            self.adam_m = {k: torch.zeros_like(v) for k, v in self.velocity.items()}
+            self.adam_v = {k: torch.zeros_like(v) for k, v in self.velocity.items()}
+            self._md, self._vvd = _descs(self.adam_m), _descs(self.adam_v)
+            self.lib.call("cz_train_set_adam", self._h, self._md, len(self.adam_m), self._vvd, len(self.adam_v),
+                          float(beta_1), float(beta_2), float(epsilon))
         self.losses = torch.zeros(4, dtype=torch.float32, device=self.device)
         self._engine = None
 
@@ -72,7 +85,8 @@ class Trainer:
         tc, mc = self.config.trainer, self.config.model
         hp = CzTrainHparams()
         hp.struct_bytes = C.sizeof(CzTrainHparams)
-        hp.lr, hp.momentum = float(lr), float(tc.momentum)
+        hp.lr = float(lr)
+        hp.momentum = 0.0 if self.optimizer == "adam" else float(tc.momentum)      # Adam ignores it
         hp.w_policy, hp.w_value = (float(x) for x in tc.loss_weights)
         hp.l2 = float(mc.l2_reg)
         return hp
@@ -93,6 +107,13 @@ class Trainer:
 
     def step(self, planes, policy, value, lr):
         return self.step_async(planes, policy, value, lr).cpu().numpy().astype(np.float64)
+
+    @property
+    def iterations(self):
+        """Adam's step counter (Keras `iterations`): steps run since this trainer was built."""
+        it = C.c_int64(0)
+        self.lib.call("cz_train_adam_iterations", self._h, C.byref(it))
+        return it.value
 
     def grad(self, name):
         """The last step's gradient of one trainable weight (loss terms, without L2) — tests."""

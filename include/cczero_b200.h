@@ -71,6 +71,25 @@ int cz_env_check_catch(const uint8_t* boards_dev, const uint16_t* moves_dev, int
 int cz_env_keys(const uint8_t* boards_dev, int n, uint64_t* keys_dev /* [n][2] */, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Human game records — worker/sl.py load_game :124-174 and worker/sl_onegreen.py load_game :134-175, one warp per game
+ * ---------------------------------------------------------------------------------------- */
+enum { CZ_SL_WXF = 0, CZ_SL_ONEGREEN = 1 };
+enum { CZ_SL_OK = 0, CZ_SL_FAILED = 1 };   /* FAILED: the reference raises on this game, or (onegreen) drops it */
+enum { CZ_SL_GAME_FIELDS = 6 };
+/* Replays n games on the light board of the reference.  init_boards_dev [n][96]: the start position in the light board's
+ * frame (y = 0 red's back rank, red pieces codes 1..7, black 9..15).  ply_offsets_dev [n + 1]: game g owns plies
+ * [off[g], off[g+1]).  plies_dev [P][4]: the WXF characters ("C2.5", "H8+7", "R+.1"; missing characters 0) or the four
+ * onegreen digits.  sides_dev [P]: +1 for a move of the red list, -1 for the black list (build_policy's flip).
+ * lut_dev [90*90]: cz_action_labels' table.  Outputs per ply: boards_out_dev [P][96] the mover-relative observation
+ * before the move (engine layout), labels_out_dev [P] the label in the mover's frame or -1 where the move has none.
+ * game_out_dev [n][CZ_SL_GAME_FIELDS] int32 = {plies applied, status, first ply not in movegen's list or -1,
+ * evaluate's ans and tot on the final observation, 1 if red is to move at the end}.  Plies after a failure are not
+ * written. */
+int cz_sl_replay(const uint8_t* init_boards_dev, const int32_t* ply_offsets_dev, const uint8_t* plies_dev,
+                 const int8_t* sides_dev, int n, int mode, const int16_t* lut_dev, uint8_t* boards_out_dev,
+                 int16_t* labels_out_dev, int32_t* game_out_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Search engine — agent/player.py (CChessPlayer) for many concurrent games
  * ---------------------------------------------------------------------------------------- */
 typedef struct cz_engine cz_engine;
@@ -388,6 +407,18 @@ int cz_train_step(cz_trainer* t, const float* planes_dev, const float* policy_ta
 /* Tests: copy the last step's gradient of one trainable weight (loss terms only, without the L2 part).  CZ_ERR_ARG:
  * unknown name or numel differs.  Synchronises; off the step path. */
 int cz_train_read_grad(cz_trainer* t, const char* name, void* dst_dev, int64_t numel);
+/* Switches the trainer to Keras 2.0.8 Adam (decay 0; worker/sl.py, worker/sl_onegreen.py).  m / v: one f32 tensor per
+ * trainable weight, named and sized like the velocity of cz_train_set_params; cz_train_step updates them IN PLACE, reads
+ * hp->lr as Keras' base lr and ignores hp->momentum.  Every trainable tensor is updated by ONE fused launch:
+ *   t = iterations + 1;  lr_t = fp32(lr * (sqrt(1 - beta_2^t) / (1 - beta_1^t)))  (float64)
+ *   g = grad + 2 l2 K (kernels only);  m = b1 m + (1 - b1) g;  v = b2 v + (1 - b2) g g;  w -= (lr_t m) / (sqrt(v) + eps)
+ * in fp32 without contraction, b1 = fp32(beta_1), 1 - b1 in fp32.  Resets iterations to 0; every successful
+ * cz_train_step adds 1.  A later cz_train_set_params returns the trainer to SGD.  CZ_ERR_STATE: no parameters set;
+ * CZ_ERR_ARG: a moment is missing or mis-sized, or beta / epsilon out of range. */
+int cz_train_set_adam(cz_trainer* t, const cz_tensor_desc* m, int32_t n_m, const cz_tensor_desc* v, int32_t n_v, double beta_1,
+                      double beta_2, double epsilon);
+/* Adam's step counter (Keras `iterations`).  CZ_ERR_STATE: the trainer uses SGD. */
+int cz_train_adam_iterations(cz_trainer* t, int64_t* iterations);
 /* Stage building blocks of the step, for parity tests (allocate scratch, synchronise):
  *   wgrad3x3  dw (Keras HWIO [3][3][c][c] f32) of a 3x3 "same" conv: x16 fp16 [n][10][9][c], dy f32 [n*90][c]
  *   dgrad3x3  dx f32 [n*90][c] = input gradient of that conv for HWIO weights w_hwio f32
