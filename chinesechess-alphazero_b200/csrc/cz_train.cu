@@ -1004,6 +1004,55 @@ int cz_train_read_grad(cz_trainer* h, const char* name, void* dst, int64_t numel
   return cz_fail(CZ_ERR_ARG, "cz_train_read_grad: no trainable tensor named %s", name);
 }
 
+// Tests: copy an intermediate buffer as the last step left it (cz_train_buffer in the header lists what each holds).
+int cz_train_read_buffer(cz_trainer* h, int32_t which, int32_t index, void* dst, int64_t dst_bytes, int64_t* bytes) {
+  if (!h) return cz_fail(CZ_ERR_ARG, "cz_train_read_buffer: null trainer");
+  Trainer* t = &h->t;
+  if (t->last_batch < 1) return cz_fail(CZ_ERR_STATE, "cz_train_read_buffer: no step has run");
+  const long long n = t->last_batch, P = n * 90, C = t->C, L = t->L;
+  const long long nbn = (long long)t->bn.size();
+  long long lim = 1;                              // valid indices are 0 .. lim - 1
+  switch (which) {
+    case CZ_TRAIN_BUF_BLOCK_OUT32: case CZ_TRAIN_BUF_BLOCK_OUT16: lim = L + 1; break;
+    case CZ_TRAIN_BUF_CONV1_OUT16: lim = L; break;
+    case CZ_TRAIN_BUF_BN_MEAN: case CZ_TRAIN_BUF_BN_VAR: case CZ_TRAIN_BUF_BN_DZ: lim = nbn; break;
+    default: break;
+  }
+  if (index < 0 || index >= lim) return cz_fail(CZ_ERR_ARG, "cz_train_read_buffer: index %d of buffer %d outside 0..%lld", index, which, lim - 1);
+  const void* src = nullptr;
+  long long nb = 0;
+  switch (which) {
+    case CZ_TRAIN_BUF_PLANE_INDEX: src = t->pl; nb = n * 2 * 90; break;
+    case CZ_TRAIN_BUF_BLOCK_OUT32: src = t->s32[index]; nb = P * C * 4; break;
+    case CZ_TRAIN_BUF_BLOCK_OUT16: src = t->a16[index]; nb = P * C * 2; break;
+    case CZ_TRAIN_BUF_CONV1_OUT16: src = t->h16[index]; nb = P * C * 2; break;
+    case CZ_TRAIN_BUF_BN_MEAN: src = t->bn[index].mean; nb = t->bn[index].C * 4LL; break;
+    case CZ_TRAIN_BUF_BN_VAR: src = t->bn[index].var; nb = t->bn[index].C * 4LL; break;
+    case CZ_TRAIN_BUF_BN_DZ: src = t->bn[index].z; nb = P * t->bn[index].C * 4; break;
+    case CZ_TRAIN_BUF_POL_FEAT: src = t->Fp; nb = n * t->pc * 90 * 4; break;
+    case CZ_TRAIN_BUF_VAL_FEAT: src = t->Fv; nb = n * t->vc * 90 * 4; break;
+    case CZ_TRAIN_BUF_LOGITS: src = t->logits; nb = n * kLabels * 4; break;
+    case CZ_TRAIN_BUF_DLOGITS: src = t->dlog; nb = n * kLabels * 4; break;
+    case CZ_TRAIN_BUF_VAL_HIDDEN_PRE: src = t->hpre; nb = n * t->H * 4; break;
+    case CZ_TRAIN_BUF_VAL_HIDDEN: src = t->hact; nb = n * t->H * 4; break;
+    case CZ_TRAIN_BUF_DVAL_HIDDEN: src = t->dh; nb = n * t->H * 4; break;
+    case CZ_TRAIN_BUF_VAL_PRE: src = t->vpre; nb = n * 4; break;
+    case CZ_TRAIN_BUF_DVAL_PRE: src = t->dvpre; nb = n * 4; break;
+    case CZ_TRAIN_BUF_CE_ROWS: src = t->ce_rows; nb = n * 4; break;
+    case CZ_TRAIN_BUF_SE_ROWS: src = t->se_rows; nb = n * 4; break;
+    case CZ_TRAIN_BUF_DPOL_FEAT: src = t->dF; nb = n * t->pc * 90 * 4; break;
+    case CZ_TRAIN_BUF_TRUNK_GRAD: src = t->G; nb = P * C * 4; break;
+    case CZ_TRAIN_BUF_SCALE_SLOTS: src = t->scale_slots; nb = (2 * L + 1) * 4 * 4; break;
+    default: return cz_fail(CZ_ERR_ARG, "cz_train_read_buffer: unknown buffer %d", which);
+  }
+  if (bytes) *bytes = nb;
+  if (!dst) return 0;
+  if (dst_bytes < nb) return cz_fail(CZ_ERR_ARG, "cz_train_read_buffer: %lld bytes < %lld", (long long)dst_bytes, nb);
+  CZ_CUDA(cudaMemcpyAsync(dst, src, (size_t)nb, cudaMemcpyDeviceToDevice, t->st));
+  CZ_CUDA(cudaStreamSynchronize(t->st));
+  return 0;
+}
+
 // ---- stage building blocks (tests): each runs the step's own launch sequence for one stage on caller buffers.
 // 3x3 conv gradients on dense activations [n][90][c]: dy f32, x fp16; dw out Keras HWIO f32 [3][3][c][c]
 int cz_train_wgrad3x3(const void* x16, const float* dy, int n, int c, float* dw, void* stream) {

@@ -141,6 +141,7 @@ _SIGS = {
     "cz_train_set_params": (C.c_int, [_P, C.POINTER(CzTensorDesc), C.c_int32, C.POINTER(CzTensorDesc), C.c_int32]),
     "cz_train_step": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.POINTER(CzTrainHparams), _P]),
     "cz_train_read_grad": (C.c_int, [_P, C.c_char_p, _P, C.c_int64]),
+    "cz_train_read_buffer": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "cz_train_set_adam": (C.c_int, [_P, C.POINTER(CzTensorDesc), C.c_int32, C.POINTER(CzTensorDesc), C.c_int32, C.c_double,
                                     C.c_double, C.c_double]),
     "cz_train_adam_iterations": (C.c_int, [_P, C.POINTER(C.c_int64)]),
@@ -150,7 +151,7 @@ _SIGS = {
 }
 # entry points that only exist in the CUDA build (tensor cores cannot be emulated on the CPU)
 CUDA_ONLY = {"cz_igemm_conv3x3", "cz_igemm_conv3x3_dense", "cz_igemm_dense", "cz_train_workspace_bytes", "cz_train_create",
-             "cz_train_destroy", "cz_train_set_params", "cz_train_step", "cz_train_read_grad", "cz_train_wgrad3x3",
+             "cz_train_destroy", "cz_train_set_params", "cz_train_step", "cz_train_read_grad", "cz_train_read_buffer", "cz_train_wgrad3x3",
              "cz_train_dgrad3x3", "cz_train_bn", "cz_train_set_adam", "cz_train_adam_iterations"}
 
 

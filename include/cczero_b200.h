@@ -407,6 +407,53 @@ int cz_train_step(cz_trainer* t, const float* planes_dev, const float* policy_ta
 /* Tests: copy the last step's gradient of one trainable weight (loss terms only, without the L2 part).  CZ_ERR_ARG:
  * unknown name or numel differs.  Synchronises; off the step path. */
 int cz_train_read_grad(cz_trainer* t, const char* name, void* dst_dev, int64_t numel);
+/* Tests: intermediate buffers of the training step, as the LAST cz_train_step left them (n = that step's batch, P = n * 90,
+ * C = filters, L = blocks, pc / vc = policy / value channels, H = value_fc).  `index` selects a block or a BN layer
+ * (0 = input, 1 + 2i + j = block i conv j + 1, 2L + 1 = policy, 2L + 2 = value) and is 0 for every other buffer.
+ *   PLANE_INDEX     int8 [n][2][90]  occupied plane 0..13 per (position, board, pixel), -1 empty (board 1: 28 planes only)
+ *   BLOCK_OUT32     f32  [P][C]      k = 0..L: output of the input conv (k = 0) / of block k, the skip stream
+ *   BLOCK_OUT16     fp16 [P][C]      k = 0..L: the same activations in fp16 (conv and wgrad operands)
+ *   CONV1_OUT16     fp16 [P][C]      i < L: relu(BN(conv1)) of block i
+ *   BN_MEAN         f32  [C_j]       batch mean of BN layer j
+ *   BN_VAR          f32  [C_j]       biased batch variance of BN layer j
+ *   BN_DZ           f32  [P][C_j]    the gradient at BN layer j's input: the backward writes dz over the conv output z
+ *   POL_FEAT        f32  [n][pc*90]  relu(BN(policy conv)) in Keras Flatten order (channel * 90 + pixel)
+ *   VAL_FEAT        f32  [n][vc*90]  the value features, same order
+ *   LOGITS, DLOGITS f32  [n][2086]   policy logits / the loss gradient at the logits (w_policy / n included)
+ *   VAL_HIDDEN_PRE  f32  [n][H]      value_dense before the ReLU
+ *   VAL_HIDDEN      f32  [n][H]      after the ReLU
+ *   DVAL_HIDDEN     f32  [n][H]      gradient at VAL_HIDDEN, masked by VAL_HIDDEN_PRE > 0 (the gradient at value_dense)
+ *   VAL_PRE         f32  [n]         value before tanh;  DVAL_PRE  f32 [n]  the loss gradient at it
+ *   CE_ROWS         f32  [n]         per-row cross-entropy;  SE_ROWS  f32 [n]  per-row squared value error
+ *   DPOL_FEAT       f32  [n][pc*90]  gradient at POL_FEAT (Flatten order); the value's feature gradient was overwritten
+ *   TRUNK_GRAD      f32  [P][C]      gradient at BLOCK_OUT32[0] (before the input BN's ReLU mask)
+ *   SCALE_SLOTS     f32  [2L+1][4]   per 3x3 conv 2i + j: {max |dz| as float bits, 2^e, 2^-e, unused} of its fp16 dz
+ * dst_dev = NULL only reports *bytes.  CZ_ERR_ARG: unknown buffer, index out of range or dst_bytes < *bytes;
+ * CZ_ERR_STATE: no step has run.  Synchronises; off the step path. */
+typedef enum cz_train_buffer {
+  CZ_TRAIN_BUF_PLANE_INDEX = 0,
+  CZ_TRAIN_BUF_BLOCK_OUT32 = 1,
+  CZ_TRAIN_BUF_BLOCK_OUT16 = 2,
+  CZ_TRAIN_BUF_CONV1_OUT16 = 3,
+  CZ_TRAIN_BUF_BN_MEAN = 4,
+  CZ_TRAIN_BUF_BN_VAR = 5,
+  CZ_TRAIN_BUF_BN_DZ = 6,
+  CZ_TRAIN_BUF_POL_FEAT = 7,
+  CZ_TRAIN_BUF_VAL_FEAT = 8,
+  CZ_TRAIN_BUF_LOGITS = 9,
+  CZ_TRAIN_BUF_DLOGITS = 10,
+  CZ_TRAIN_BUF_VAL_HIDDEN_PRE = 11,
+  CZ_TRAIN_BUF_VAL_HIDDEN = 12,
+  CZ_TRAIN_BUF_DVAL_HIDDEN = 13,
+  CZ_TRAIN_BUF_VAL_PRE = 14,
+  CZ_TRAIN_BUF_DVAL_PRE = 15,
+  CZ_TRAIN_BUF_CE_ROWS = 16,
+  CZ_TRAIN_BUF_SE_ROWS = 17,
+  CZ_TRAIN_BUF_DPOL_FEAT = 18,
+  CZ_TRAIN_BUF_TRUNK_GRAD = 19,
+  CZ_TRAIN_BUF_SCALE_SLOTS = 20
+} cz_train_buffer;
+int cz_train_read_buffer(cz_trainer* t, int32_t which, int32_t index, void* dst_dev, int64_t dst_bytes, int64_t* bytes);
 /* Switches the trainer to Keras 2.0.8 Adam (decay 0; worker/sl.py, worker/sl_onegreen.py).  m / v: one f32 tensor per
  * trainable weight, named and sized like the velocity of cz_train_set_params; cz_train_step updates them IN PLACE, reads
  * hp->lr as Keras' base lr and ignores hp->momentum.  Every trainable tensor is updated by ONE fused launch:

@@ -278,12 +278,12 @@ def split_pol_feat(pf, pol_k1):
 
 # ---------------------------------------------------------------------------------------------- test nets and positions
 
-def well_conditioned_weights(filters, blocks, planes, seed=0, logit_std=2.0, value_pre=0.5, device="cpu", **kw):
+def well_conditioned_weights(filters, blocks, planes, seed=0, logit_std=2.0, value_pre=0.5, device="cpu", value_fc=256, **kw):
     """om.init_weights(trained_like=True, spread=0.3) with policy_out rescaled so that the per-row standard deviation of the
     float64 logits on `planes` averages `logit_std`, and value_out rescaled so that the median |value_pre| is `value_pre`:
     probabilities spread over several orders of magnitude and values on the steep part of tanh, where a kernel error
     is visible instead of hidden under a near-uniform 2086-way softmax or tanh's flat tails."""
-    w = om.init_weights(filters, blocks, 256, seed=seed, trained_like=True, spread=0.3, **kw)
+    w = om.init_weights(filters, blocks, value_fc, seed=seed, trained_like=True, spread=0.3, **kw)
     st = om.forward_stages(w, planes, blocks, device=device)
     a = logit_std / st["logits"].std(dim=1).mean().item()
     b = value_pre / st["value_pre"].abs().median().item()

@@ -5,12 +5,14 @@ a proof for every bound that it rejects a subtly wrong kernel (assert_rejects).
 Gradient operands of the tensor-core convolutions are fp16 times a power of two 2^e with max|dy| 2^e in [2^14, 2^15);
 the references below take exactly those operands (scaling is exact), so what is measured is the accumulation.
 
-wgrad's K is the batch's pixel count, up to 92 160 at batch 1024, 40x the forward's 2304.  Each CTA accumulates one
-contiguous split of at most ceil(chunks / splits) * 64 pixels (about 13 200 at batch 1024, C = 256: 7 splits) in the
-wgmma fp32 accumulator, then <= 14 split partials are summed in fp32 in a fixed order.  The forward's BETA = 2^-16
-carries a 5x margin over sqrt(K) 2^-24 S at K = 2304; the same argument at K = 13 200 gives sqrt(13 200) 2^-24 S =
-2^-17.2 S for the accumulator and 14 * 2^-24 S = 2^-20.2 S for the ordered split sum, so WGRAD_BETA = 2^-13 keeps a
->10x margin.  One board-edge column missing from a tap drops about 1/9 of its terms (~0.1 S), far above it.
+wgrad's K is the batch's pixel count, up to 368 640 at max_batch 4096, 160x the forward's 2304.  Each CTA accumulates
+one contiguous split of at most ceil(chunks / splits) * 64 pixels in the wgmma fp32 accumulator, then <= 14 split
+partials are summed in fp32 in a fixed order.  On 132 SMs that is about 13 200 pixels at batch 1024, C = 256 (7 splits),
+and 52 700 at batch 4096, C = 256 (7 splits of 823 chunks; C = 64: 14 splits, 26 400 pixels).  The forward's BETA =
+2^-16 carries a 5x margin over sqrt(K) 2^-24 S at K = 2304; the same argument at K = 52 700 gives sqrt(52 700) 2^-24 S =
+2^-16.2 S for the accumulator and 14 * 2^-24 S = 2^-20.2 S for the ordered split sum, so WGRAD_BETA = 2^-13 keeps a
+9x margin at the longest split the ABI allows (>10x up to batch 1024).  One board-edge column missing from a tap drops
+about 1/9 of its terms (~0.1 S), far above it.
 """
 import ctypes as C
 
@@ -53,7 +55,7 @@ def wgrad_ref(x16, dy16, n, c):
     return w.permute(2, 3, 1, 0).contiguous(), s.permute(2, 3, 1, 0).contiguous()
 
 
-WGRAD_CASES = [(64, 1), (64, 256), (128, 7), (192, 256), (256, 7), (256, 1024)]
+WGRAD_CASES = [(64, 1), (64, 256), (128, 7), (192, 256), (256, 7), (256, 1024), (256, 4096), (64, 4096)]
 
 
 @pytest.mark.parametrize("c,n", WGRAD_CASES)
