@@ -105,6 +105,14 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
     if (t == 0) {
       wg::prefetch_tmap(&tmA);
       wg::prefetch_tmap(&tmB);
+      // Dense conv with a skip stream: the epilogue reads the tile's skip rows right after the last MMA, when every CTA of the
+      // wave does the same, so the reads would all miss L2 at once with the tensor cores idle.  Halfway through the tile's
+      // main loop the producer prefetches them into L2 instead (rows below args_rows only; at N_TILE = ldo one contiguous
+      // range, else one range per row).  Halfway rather than at the tile's first load: the first load is issued while the
+      // previous tile's epilogue still has to stream its outputs through L2, which could evict the prefetched lines.
+      const uint8_t* skip = a.conv != 2 ? nullptr : a.residual32 ? reinterpret_cast<const uint8_t*>(a.residual32)
+                                                                 : reinterpret_cast<const uint8_t*>(a.residual);
+      const int skip_es = a.residual32 ? 4 : 2;
       uint32_t s = 0, ph = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int m_tile = tile % m_tiles, n_tile = tile / m_tiles;
@@ -114,6 +122,14 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
           const int dy = a.n_taps == 9 ? tap / 3 - 1 : 0;
           const int dx = a.n_taps == 9 ? tap % 3 - 1 : 0;
           for (int kc = 0; kc < a.k_chunks; ++kc) {
+            if (skip && tap * a.k_chunks + kc == n_kb / 2) {
+              const int nr = min(kTileM, rows - pix0);
+              const uint8_t* p0 = skip + ((long long)pix0 * a.ldo + n_tile * N_TILE) * skip_es;
+              if (N_TILE == a.ldo)
+                wg::prefetch_l2_bulk(p0, (uint32_t)(nr * N_TILE * skip_es));
+              else
+                for (int r = 0; r < nr; ++r) wg::prefetch_l2_bulk(p0 + (long long)r * a.ldo * skip_es, N_TILE * skip_es);
+            }
             wg::mbar_wait(&empty[s], ph ^ 1);
             uint8_t* sA = smem + s * C::kStageBytes;
             uint8_t* sB = sA + kAStageBytes;
@@ -167,20 +183,52 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
         acc[4 * j] += b.x; acc[4 * j + 1] += b.y; acc[4 * j + 2] += b.x; acc[4 * j + 3] += b.y;
       }
     }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
+    // accumulator row mrow + 8h: global output row, inside the batch, strip separator row (stays zero)
+    auto out_row = [&](int h, long long& grow, bool& valid, bool& zero) {
       const int m = mrow + 8 * h;                           // accumulator row == pixel / row inside the tile
-      long long grow;                                       // global output row
-      bool valid, zero = false;
+      zero = false;
       if (a.conv == 1) {
         const int srow = m_tile * a.box_r + m / 9;          // strip row
         valid = m < a.box_r * 9 && srow < rows;
-        zero = (srow % 11) == 10;                           // separator row stays zero
+        zero = (srow % 11) == 10;
         grow = (long long)m_tile * a.box_r * 9 + m;
       } else {
         grow = (long long)m_tile * kTileM + m;
         valid = grow < rows;
       }
+    };
+    // + skip stream, for both rows before the first output store.  The compiler keeps every load behind the stores that
+    // precede it (a store might alias the skip stream), so loads interleaved with the stores would go out one round trip
+    // at a time; here they go out back to back.  Same operations in the same order: (acc + bias) + skip.
+    if (!a.out_f32 && (a.residual32 || a.residual)) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        long long grow;
+        bool valid, zero;
+        out_row(h, grow, valid, zero);
+        if (!valid) continue;
+        if (a.residual32) {
+          const float* r32 = a.residual32 + grow * a.ldo;
+#pragma unroll
+          for (int j = 0; j < N_TILE / 8; ++j) {
+            const float2 r = __ldg(reinterpret_cast<const float2*>(r32 + nb + 8 * j));
+            acc[4 * j + 2 * h] += r.x; acc[4 * j + 2 * h + 1] += r.y;
+          }
+        } else {
+          const __half* r16 = a.residual + grow * a.ldo;
+#pragma unroll
+          for (int j = 0; j < N_TILE / 8; ++j) {
+            const float2 r = __half22float2(__ldg(reinterpret_cast<const __half2*>(r16 + nb + 8 * j)));
+            acc[4 * j + 2 * h] += r.x; acc[4 * j + 2 * h + 1] += r.y;
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      long long grow;                                       // global output row
+      bool valid, zero;
+      out_row(h, grow, valid, zero);
       if (a.out_f32) {
         if (a.row_stats) {                                  // the 4 threads of a quad hold one row: reduce across them
           float mx = -INFINITY;
@@ -214,15 +262,11 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
       } else {
         if (!valid) continue;
         __half* o = reinterpret_cast<__half*>(a.out) + grow * a.ldo;
-        const float* r32 = a.residual32 ? a.residual32 + grow * a.ldo : nullptr;
-        const __half* r16 = (!a.residual32 && a.residual) ? a.residual + grow * a.ldo : nullptr;
         float* o32 = a.out32 ? a.out32 + grow * a.ldo : nullptr;
 #pragma unroll
         for (int j = 0; j < N_TILE / 8; ++j) {
           const int n = nb + 8 * j;
           float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
-          if (r32) { const float2 r = __ldg(reinterpret_cast<const float2*>(r32 + n)); x0 += r.x; x1 += r.y; }
-          else if (r16) { const float2 r = __half22float2(__ldg(reinterpret_cast<const __half2*>(r16 + n))); x0 += r.x; x1 += r.y; }
           if (a.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
           if (zero) { x0 = 0.f; x1 = 0.f; }
           *reinterpret_cast<__half2*>(o + n) = __floats2half2_rn(x0, x1);

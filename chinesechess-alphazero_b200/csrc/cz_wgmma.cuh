@@ -50,6 +50,11 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* t, uin
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(t)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// Bulk prefetch of [p, p + bytes) into L2 (16-byte aligned, bytes a multiple of 16).  Nothing waits for it: a later load of
+// the range hits L2 if the lines are still there.
+__device__ __forceinline__ void prefetch_l2_bulk(const void* p, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"((uint64_t)__cvta_generic_to_global(p)), "r"(bytes) : "memory");
+}
 // im2col-mode load: {c, w, h, n} is the base pixel (output pixel minus padding), {ow, oh} the filter tap.
 __device__ __forceinline__ void tma_load_im2col_4d(void* dst, const CUtensorMap* t, uint64_t* bar, int c, int w, int h, int n,
                                                    uint16_t ow, uint16_t oh) {
