@@ -20,6 +20,14 @@
 //   on its 64 rows of the tile with fp32 accumulators in registers, then running the epilogue from those registers
 //   (+bias (+residual) -> ReLU -> fp16 / fp32 -> HBM).  kStages-deep smem ring with full/empty mbarriers; the producer runs
 //   ahead into the next tile while the consumers store the current one.  Persistent: grid <= #SMs, tiles strided over CTAs.
+//   After the role split the producer warpgroup gives its registers to the consumers (setmaxnreg).
+// Staged epilogue (Args::staged: dense conv without a skip stream, fp16 out, M tiles that lie wholly inside the batch): the
+//   tile leaves in 32-column steps through a small ring of slots per consumer warpgroup.  A slot holds 64 rows x 32 fp16
+//   columns (64-byte rows, SWIZZLE_64B, as the output's tensor map expects); the warpgroup writes a step into a slot and one
+//   thread hands it to a TMA store, so the stores are whole sectors and drain while the next tile's MMAs run.  The arithmetic
+//   per element is that of the register epilogue, which everything else keeps: the convs with a skip stream (loading it by
+//   TMA into the ring was measured and did not pay, DESIGN.md 3.1), and the last, partial M tile, because a tensor store
+//   clips at the buffer's extent, not at the device-side batch.
 #pragma once
 #include <cuda_fp16.h>
 #include "cz_wgmma.cuh"
@@ -33,6 +41,10 @@ constexpr int kThreads = 384;
 constexpr int kConsumerWarps = 8;
 constexpr int kSmemLimit = 232448;          // opt-in dynamic shared memory per CTA on sm_90 (227 KB)
 constexpr int kMaxStages = 8;
+constexpr int kEpiCols = 32;                       // columns per step of the staged epilogue
+constexpr int kEpiSlotBytes = 64 * kEpiCols * 2;   // 4 KB: 64 rows x 32 fp16
+constexpr int kEpiSlots = 3;                       // per consumer warpgroup: one being written, two being stored
+constexpr int kEpiBytes = kEpiSlots * kEpiSlotBytes;
 
 struct Args {
   int n_taps;        // 9 (3x3 conv) or 1 (plain GEMM)
@@ -61,34 +73,41 @@ struct Args {
   // GEMM mode (out_f32): per output row and N tile the pair {max_j x_j, sum_j exp(x_j - max)} over the tile's valid
   // columns — the softmax is finished by whoever reads the logits (k_softmax / k_legal_priors), never a second full pass
   float2* row_stats; // [rows][n_tiles] or null
+  int staged;        // dense conv, fp16 out, no skip: tmOut is valid, full M tiles take the staged epilogue
 };
 
 // rows / m-tiles of this launch (device-side batch size)
 __device__ __forceinline__ int args_rows(const Args& a) { return a.n_dev ? __ldg(a.n_dev) * a.rows_per_unit : a.rows; }
 
+// Shared memory: the epilogue ring of both consumer warpgroups, then as many operand stages as still fit
 template <int N_TILE>
 struct Cfg {
   static constexpr int kBStageBytes = N_TILE * 128;
   static constexpr int kStageBytes = kAStageBytes + kBStageBytes;
-  static constexpr int kFit = (kSmemLimit - 256 - 1024) / kStageBytes;
+  static constexpr int kFit = (kSmemLimit - 2 * kEpiBytes - 256 - 1024) / kStageBytes;
   static constexpr int kStages = kFit > kMaxStages ? kMaxStages : kFit;   // 4 (N = 256) .. 8 (N = 64)
-  static constexpr int kSmemBytes = kStages * kStageBytes + 256 + 1024;    // + barriers + alignment slack
+  static constexpr int kSmemBytes = kStages * kStageBytes + 2 * kEpiBytes + 256 + 1024;    // + barriers + alignment slack
   static_assert(N_TILE % 64 == 0 && N_TILE <= 256, "wgmma N tile");
+  static_assert((2 * kStages + 2 * kEpiSlots) * 8 <= 256, "barrier space");
 };
 
 template <int N_TILE>
 __global__ void __launch_bounds__(kThreads, 1)
-k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Args a) {
+k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
+        const Args a) {
   using C = Cfg<N_TILE>;
   constexpr int S = C::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * C::kStageBytes);   // [S]  TMA -> MMA
+  uint8_t* epi = smem + S * C::kStageBytes;                                   // [2 warpgroups][kEpiBytes]
+  uint64_t* full = reinterpret_cast<uint64_t*>(epi + 2 * kEpiBytes);          // [S]  TMA -> MMA
   uint64_t* empty = full + S;                                                 // [S]  MMA -> TMA (one arrive per consumer warp)
+  uint64_t* efree = empty + S;    // [2][kEpiSlots]  the slot's last store has read it: the warpgroup may write it again
 
   const int wgi = threadIdx.x >> 7, t = threadIdx.x & 127;
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) { wg::mbar_init(&full[s], 1); wg::mbar_init(&empty[s], kConsumerWarps); }
+    for (int s = 0; s < 2 * kEpiSlots; ++s) wg::mbar_init(&efree[s], 1);
     wg::fence_barrier_init();
   }
   wg::griddep_launch_dependents();     // (PDL launches only) the next conv may become resident while this one runs
@@ -100,8 +119,12 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
   const int m_tiles = a.conv == 1 ? a.m_tiles : (rows + kTileM - 1) / kTileM;
   const int total_tiles = m_tiles * a.n_tiles;
 
+  constexpr int kSteps = N_TILE / kEpiCols;                // steps of the staged epilogue per tile
+  auto tile_staged = [&](int tile) { return a.staged && (tile % m_tiles) * kTileM + kTileM <= rows; };
+
   if (wgi == 0) {
     // ------------------------------------------------------------ TMA producer
+    wg::reg_dealloc<40>();
     if (t == 0) {
       wg::prefetch_tmap(&tmA);
       wg::prefetch_tmap(&tmB);
@@ -148,10 +171,25 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
   }
 
   // -------------------------------------------------------------- consumers: MMA + epilogue on rows cw*64 .. cw*64+63
+  wg::reg_alloc<232>();
   const int cw = wgi - 1, warp = t >> 5, lane = t & 31;
   const int mrow = cw * 64 + warp * 16 + (lane >> 2);       // accumulator rows mrow and mrow + 8 of the tile
   const int cq = 2 * (lane & 3);                            // first of the two adjacent columns per 8-column group
   float acc[N_TILE / 2];
+  // staged epilogue: this warpgroup's slots and barriers; byte offset of this thread's first row (warp * 16 + lane / 4 of the
+  // warpgroup's 64; the second is 8 rows on, same swizzle phase) and column pair inside a slot, before the swizzle XOR
+  uint8_t* ering = epi + cw * kEpiBytes;
+  uint64_t* fre = efree + cw * kEpiSlots;
+  const uint32_t erow = warp * 16 + (lane >> 2);
+  const uint32_t e_off = erow * 64 + (lane & 3) * 4, e_x = (erow >> 1) & 3;
+  uint32_t e_slot = 0, e_ph = 0;                              // the next step's slot and its parity
+  uint32_t e_issued = 0, e_released = 0, e_rel_slot = 0;      // (thread 0 of the warpgroup) steps stored / slots handed back
+  auto release_to = [&](uint32_t upto) {                      // the stores of steps < upto have read their slots
+    for (; e_released < upto; ++e_released) {
+      wg::mbar_arrive(&fre[e_rel_slot]);
+      if (++e_rel_slot == kEpiSlots) e_rel_slot = 0;
+    }
+  };
   uint32_t s = 0, ph = 0;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     const int m_tile = tile % m_tiles, n_tile = tile / m_tiles;
@@ -182,6 +220,36 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
         const float2 b = __ldg(reinterpret_cast<const float2*>(a.bias + nb + 8 * j));
         acc[4 * j] += b.x; acc[4 * j + 1] += b.y; acc[4 * j + 2] += b.x; acc[4 * j + 3] += b.y;
       }
+    }
+    if (tile_staged(tile)) {
+      if (t == 0) { wg::bulk_wait_group_read<0>(); release_to(e_issued); }    // the previous tile's last slots
+#pragma unroll
+      for (int st = 0; st < kSteps; ++st) {
+        uint8_t* slot = ering + e_slot * kEpiSlotBytes;
+        wg::mbar_wait(&fre[e_slot], e_ph ^ 1);              // passes on a slot that has not been used yet
+#pragma unroll
+        for (int jj = 0; jj < kEpiCols / 8; ++jj) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int i = 4 * (st * (kEpiCols / 8) + jj) + 2 * h;
+            float x0 = acc[i], x1 = acc[i + 1];
+            if (a.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
+            *reinterpret_cast<__half2*>(slot + e_off + h * 8 * 64 + ((jj ^ e_x) << 4)) = __floats2half2_rn(x0, x1);
+          }
+        }
+        wg::fence_proxy_async();
+        wg::named_barrier(1 + cw, 128);
+        if (t == 0) {
+          wg::tma_store_2d(&tmOut, slot, n_tile * N_TILE + st * kEpiCols, m_tile * kTileM + cw * 64);
+          wg::bulk_commit();
+          ++e_issued;
+          // hand back the previous step's slot (its store has had this step's time to read it); this step's store stays in flight
+          wg::bulk_wait_group_read<1>();
+          release_to(e_issued - 1);
+        }
+        if (++e_slot == kEpiSlots) { e_slot = 0; e_ph ^= 1; }
+      }
+      continue;
     }
     // accumulator row mrow + 8h: global output row, inside the batch, strip separator row (stays zero)
     auto out_row = [&](int h, long long& grow, bool& valid, bool& zero) {
@@ -275,6 +343,7 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
       }
     }
   }
+  if (t == 0) wg::bulk_wait_group_all();                    // the staged stores have landed before the grid can count as complete
 }
 
 }  // namespace igemm

@@ -112,6 +112,20 @@ int make_map_2d(CUtensorMap* m, const void* base, int k, long long rows, int box
   return 0;
 }
 
+// fp16 matrix [rows][cols] as the staged conv epilogue stores it: boxes of 32 columns x 64 rows, 64-byte rows in shared memory
+static int make_map_epi(CUtensorMap* m, const void* base, int cols, long long rows) {
+  if (load_encode()) return CZ_ERR_CUDA;
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
+  cuuint32_t box[2] = {(cuuint32_t)igemm::kEpiCols, 64};
+  cuuint32_t es[2] = {1, 1};
+  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return cz_fail(CZ_ERR_CUDA, "cuTensorMapEncodeTiled(epilogue) failed: %d", (int)r);
+  return 0;
+}
+
 static int g_num_sms = 0;
 int num_sms() {
   if (!g_num_sms) {
@@ -132,7 +146,7 @@ static bool use_pdl() {
   return pdl == 1;
 }
 template <int N_TILE>
-static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const igemm::Args& a, cudaStream_t st) {
+static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut, const igemm::Args& a, cudaStream_t st) {
   using C = igemm::Cfg<N_TILE>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -150,19 +164,24 @@ static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const 
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     lc.attrs = at; lc.numAttrs = 1;
-    CZ_CUDA(cudaLaunchKernelEx(&lc, igemm::k_igemm<N_TILE>, tmA, tmB, a));
+    CZ_CUDA(cudaLaunchKernelEx(&lc, igemm::k_igemm<N_TILE>, tmA, tmB, tmOut, a));
   } else {
-    igemm::k_igemm<N_TILE><<<grid, igemm::kThreads, C::kSmemBytes, st>>>(tmA, tmB, a);
+    igemm::k_igemm<N_TILE><<<grid, igemm::kThreads, C::kSmemBytes, st>>>(tmA, tmB, tmOut, a);
   }
   CZ_CUDA(cudaGetLastError());
   return 0;
 }
-int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, const igemm::Args& a, cudaStream_t st) {
+// With `out_map` (make_map_epi of a.out) the full M tiles of a dense conv that has fp16 output only and no skip stream leave
+// through the staged epilogue.
+int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, const igemm::Args& a0, cudaStream_t st, const CUtensorMap* out_map) {
+  igemm::Args a = a0;
+  a.staged = out_map && a.conv == 2 && !a.out_f32 && !a.residual && !a.residual32 && !a.out32;
+  const CUtensorMap& tmOut = a.staged ? *out_map : tmA;    // not used unless staged
   switch (n_tile) {
-    case 64: return launch_igemm_t<64>(tmA, tmB, a, st);
-    case 128: return launch_igemm_t<128>(tmA, tmB, a, st);
-    case 192: return launch_igemm_t<192>(tmA, tmB, a, st);
-    case 256: return launch_igemm_t<256>(tmA, tmB, a, st);
+    case 64: return launch_igemm_t<64>(tmA, tmB, tmOut, a, st);
+    case 128: return launch_igemm_t<128>(tmA, tmB, tmOut, a, st);
+    case 192: return launch_igemm_t<192>(tmA, tmB, tmOut, a, st);
+    case 256: return launch_igemm_t<256>(tmA, tmB, tmOut, a, st);
   }
   return cz_fail(CZ_ERR_UNSUPPORTED, "igemm: unsupported N tile %d (filters must be 64/128/192/256)", n_tile);
 }
@@ -550,6 +569,7 @@ struct NnRuntime {
   bool fp32_skip;                        // keep the residual (skip) stream in fp32: halves the value error of deep nets, ~+30 % time
   int board_pixels;                      // 99 = strip layout (separator row per board), 90 = dense + im2col TMA
   CUtensorMap imap_x, imap_t, imap_y;    // im2col maps of the three activation buffers (dense layout)
+  CUtensorMap emap_t;                    // conv1's output buffer as the staged conv epilogue stores it
   // optional CUDA-event timing of the residual-tower launches (bench.py roofline)
   bool profile;
   std::vector<cudaEvent_t> ev;        // pairs, recycled
@@ -666,6 +686,7 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
     rc |= make_map_im2col(&r->imap_x, r->x, c, max_batch);
     rc |= make_map_im2col(&r->imap_t, r->t, c, max_batch);
     rc |= make_map_im2col(&r->imap_y, r->y, c, max_batch);
+    rc |= make_map_epi(&r->emap_t, r->t, c, (long long)max_batch * 90);
   }
   rc |= make_map_3d(&r->map_x, r->x, c, 9, rows, 9, 14);
   rc |= make_map_3d(&r->map_t, r->t, c, 9, rows, 9, 14);
@@ -860,7 +881,7 @@ static int fw_tower(NnRuntime* r, int n, const int* n_dev) {
       const int nt = split ? 64 : c;
       const std::vector<CUtensorMap>& wm = split ? r->map_w_64 : r->map_w;
       d1.n_tiles = d2.n_tiles = c / nt;
-      if (launch_igemm(nt, *ix, wm[2 * i], d1, st)) return CZ_ERR_CUDA;
+      if (launch_igemm(nt, *ix, wm[2 * i], d1, st, &r->emap_t)) return CZ_ERR_CUDA;
       if (launch_igemm(nt, r->imap_t, wm[2 * i + 1], d2, st)) return CZ_ERR_CUDA;
       CUtensorMap* ti = ix; ix = iy; iy = ti;
     } else {

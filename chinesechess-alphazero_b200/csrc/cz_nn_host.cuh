@@ -13,7 +13,9 @@ int make_map_im2col(CUtensorMap* m, const void* base, int c, long long n_images,
 // fp16 matrix [rows][k] (k contiguous), box {64, box_rows}, 128-byte swizzle, zero OOB fill
 int make_map_2d(CUtensorMap* m, const void* base, int k, long long rows, int box_rows);
 int num_sms();
-// igemm::k_igemm<n_tile> on `st` (n_tile 64 / 128 / 192 / 256)
-int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, const igemm::Args& a, cudaStream_t st);
+// igemm::k_igemm<n_tile> on `st` (n_tile 64 / 128 / 192 / 256).  `out_map`: tensor map of a.out for the staged epilogue of a
+// dense conv with fp16 output and no skip stream (Args::staged is set from it); null: register epilogue.
+int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, const igemm::Args& a, cudaStream_t st,
+                 const CUtensorMap* out_map = nullptr);
 
 }  // namespace cznn

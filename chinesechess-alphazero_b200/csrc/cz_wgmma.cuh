@@ -34,6 +34,18 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   } while (!ok);
 }
 
+// ---------------------------------------------------------------- warp-specialised CTAs
+// Barrier `id` (1..15; 0 is __syncthreads) over `threads` threads: the warps of one role, when the roles have diverged.
+__device__ __forceinline__ void named_barrier(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// Give back / take registers, by every thread of a warpgroup: the per-thread limit becomes N (a multiple of 8).  The
+// increase waits until other warpgroups have released enough.
+template <int N>
+__device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* t) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(t)) : "memory");
@@ -50,6 +62,20 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* t, uin
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(t)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+// Tensor store shared -> global of one box at {c0, c1}.  Stores are tracked in the issuing thread's bulk groups: commit, then
+// wait_group_read<N> until all but the N latest groups have finished READING shared memory (the source may be rewritten; the
+// data need not have landed), or wait_group_all until every group is complete (before the thread exits).
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* t, const void* src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(t)), "r"(smem_u32(src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// Generic-proxy writes to shared memory become visible to the async proxy (a TMA store that reads them).
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // Bulk prefetch of [p, p + bytes) into L2 (16-byte aligned, bytes a multiple of 16).  Nothing waits for it: a later load of
 // the range hits L2 if the lines are still there.
 __device__ __forceinline__ void prefetch_l2_bulk(const void* p, uint32_t bytes) {

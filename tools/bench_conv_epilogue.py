@@ -6,6 +6,10 @@ do the same MMAs; conv2's epilogue additionally reads the skip stream and writes
 activations stream from HBM) and at batch 1024 (they stay in L2), so a gap that is the epilogue's HBM traffic shows up as
 conv2 > conv1 at 8192 and shrinks at 1024.
 
+Each row also carries the MMA-only lower bound of a launch at the sampled median SM clock, from shapes alone: the waves of
+128 x N tiles over the SMs times 2 * 128 * N * 9C FLOP per tile, at 4096 dense fp16 FLOP per clock per SM.  What a tile takes
+beyond that bound is conv1's main-loop plus epilogue loss; what conv2 takes beyond conv1 is its epilogue's.
+
     python tools/bench_conv_epilogue.py [--filters 256] [--blocks 20] [--batches 8192,1024] [--out DIR]
 """
 import argparse
@@ -26,6 +30,7 @@ from oracle import model as om
 from oracle import senv
 
 TILE_M = 128
+SM_FLOP_PER_CLK = 4096          # dense fp16 tensor-core FLOP per clock per SM (H100 data sheet: 989 TFLOP/s, 132 SMs, 1830 MHz)
 
 
 def smi(fields):
@@ -64,10 +69,10 @@ def measure(lib, filters, blocks, batch, forwards, seed):
         clk_out, _ = sampler.communicate(timeout=30)
     eng.close()
     clocks = [int(x) for x in clk_out.split() if x.strip().isdigit()]
-    name = f"k_igemm<{filters}>"
+    name = f"k_igemm<{filters}"
     ev = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and name in e.name),
                 key=lambda e: e.time_range.start)
-    per_fwd = 2 * blocks + 1                       # the tower's convs, then the policy GEMM (same template, GEMM mode)
+    per_fwd = 2 * blocks + (filters == 256)        # the tower's convs, then the policy GEMM (same template at N = 256)
     assert len(ev) == forwards * per_fwd, (len(ev), forwards, per_fwd)
     us1, us2 = [], []
     for f in range(forwards):
@@ -85,6 +90,13 @@ def measure(lib, filters, blocks, batch, forwards, seed):
     row["conv2_over_conv1"] = round(row["conv2"]["median_us"] / row["conv1"]["median_us"], 3)
     row["sm_clock_mhz"] = {"median": statistics.median(clocks) if clocks else None, "min": min(clocks, default=None),
                            "max": max(clocks, default=None), "samples": len(clocks)}
+    if clocks:
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
+        waves = (tiles + sms - 1) // sms
+        tile_us = 2.0 * TILE_M * filters * 9 * filters / (SM_FLOP_PER_CLK * row["sm_clock_mhz"]["median"])
+        row["mma_bound"] = {"waves": waves, "tile_us": round(tile_us, 2), "launch_us": round(waves * tile_us, 1)}
+        for tag in ("conv1", "conv2"):
+            row[tag]["tile_excess_us"] = round(row[tag]["median_us"] / waves - tile_us, 2)
     return row
 
 
@@ -109,6 +121,10 @@ def main():
             print(f"  {tag}: {c['median_us']:8.1f} us median [{c['min_us']}, {c['max_us']}] over {c['launches']}  {c['tflops']:6.1f} TFLOP/s"
                   f"  HBM bytes/tile {c['hbm_bytes_per_tile']}  ({c['hbm_gb_s']} GB/s)")
         print(f"  conv2 / conv1 = {r['conv2_over_conv1']}")
+        if "mma_bound" in r:
+            b = r["mma_bound"]
+            print(f"  MMA-only bound at that clock: {b['launch_us']} us per launch ({b['waves']} waves x {b['tile_us']} us per tile);"
+                  f" per-tile excess conv1 {r['conv1']['tile_excess_us']} us, conv2 {r['conv2']['tile_excess_us']} us")
     print("card, power limit, max SM clock:", card)
     print(json.dumps(res))
     if args.out:
