@@ -1,4 +1,5 @@
-// cz_replay.cu — replay of human game records on the rules board, one warp per game (cz_sl_replay).
+// cz_replay.cu — replay of human game records on the rules board, one warp per game (cz_sl_replay), and of the
+// project's own self-play records (cz_play_replay, at the end of the file).
 //
 // Restates what the reference's supervised workers feed Keras: worker/sl.py load_game :124-174 (WXF moves resolved on the
 // light board, light_env/chessboard.py parse_WXF_move :312-356 and find_row :358-398) and worker/sl_onegreen.py
@@ -208,9 +209,51 @@ CZ_KERNEL(k_sl_replay)(const uint8_t* init, const int32_t* offs, const uint8_t* 
   }
 }
 
+// Self-play records (cz_play_replay): the board is the engine's mover-relative board throughout, and a ply is exactly
+// senv.step (static_env.py:79-86, step + fliped_state), i.e. step_flip, applied unchecked like records.expanding_data
+// applies it through cz_env_step.
+struct PlaySmem {
+  uint8_t board[BOARD_STRIDE];
+};
+
+CZ_KERNEL(k_play_replay)(const uint8_t* init, const int32_t* offs, const uint16_t* moves, int n, const int16_t* lut,
+                         uint8_t* boards_out, int16_t* labels_out, int32_t* status_out) {
+  const int g = czs::block_idx() * czs::warps_per_block() + czs::warp_in_block();
+  if (g >= n) return;
+  uint8_t* b = (reinterpret_cast<PlaySmem*>(czs::dyn_smem()) + czs::warp_in_block())->board;
+  for (int k = czs::lane(); k < BOARD_STRIDE; k += 32) b[k] = k < NSQ ? init[(size_t)g * BOARD_STRIDE + k] : 0;
+  czs::syncwarp();
+  const int o0 = offs[g], o1 = offs[g + 1];
+  int status = CZ_PLAY_OK;
+  for (int o = o0; o < o1; ++o) {
+    const move_t m = moves[o];
+    const bool on_board = mv_from(m) < NSQ && mv_to(m) < NSQ;
+    const int lab = on_board ? lut[mv_from(m) * 90 + mv_to(m)] : -1;
+    if (czs::lane() < BOARD_STRIDE / 16)
+      reinterpret_cast<uint4*>(boards_out + (size_t)o * BOARD_STRIDE)[czs::lane()] = reinterpret_cast<const uint4*>(b)[czs::lane()];
+    if (czs::lane() == 0) labels_out[o] = (int16_t)lab;
+    if (lab < 0) { status = CZ_PLAY_FAILED; break; }       // expanding_data raises: "move ... is not an action label"
+    step_flip(b, m, b);                                    // reads the board, syncs the warp, then writes it
+  }
+  if (czs::lane() == 0) status_out[g] = status;
+}
+
 }  // namespace
 
 extern "C" {
+
+int cz_play_replay(const uint8_t* init_boards, const int32_t* ply_offsets, const uint16_t* moves, int n, const int16_t* lut,
+                   uint8_t* boards_out, int16_t* labels_out, int32_t* status_out, void* stream) {
+  if (n < 0) return cz_fail(CZ_ERR_ARG, "cz_play_replay: bad n");
+  if (n == 0) return CZ_OK;
+  if (!init_boards || !ply_offsets || !lut || !status_out) return cz_fail(CZ_ERR_ARG, "cz_play_replay: null argument");
+  CZ_LAUNCH(k_play_replay, (n + kWarpsPerBlock - 1) / kWarpsPerBlock, kWarpsPerBlock, sizeof(PlaySmem) * kWarpsPerBlock,
+            (cz_stream_t)stream, init_boards, ply_offsets, moves, n, lut, boards_out, labels_out, status_out);
+  const char* msg;
+  const int e = czrt_last_error(&msg);
+  if (e) return cz_fail(CZ_ERR_CUDA, "cz_play_replay: %s", msg);
+  return CZ_OK;
+}
 
 int cz_sl_replay(const uint8_t* init_boards, const int32_t* ply_offsets, const uint8_t* plies, const int8_t* sides, int n,
                  int mode, const int16_t* lut, uint8_t* boards_out, int16_t* labels_out, int32_t* game_out, void* stream) {

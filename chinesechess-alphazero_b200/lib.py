@@ -92,6 +92,7 @@ _SIGS = {
     "cz_env_check_catch": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P]),
     "cz_env_keys": (C.c_int, [_P, C.c_int, _P, _P]),
     "cz_sl_replay": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
+    "cz_play_replay": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, _P]),
     "cz_workspace_bytes": (C.c_int, [C.POINTER(CzConfig), C.POINTER(C.c_uint64)]),
     "cz_create": (C.c_int, [C.POINTER(CzConfig), _P, C.c_uint64, _P, C.POINTER(_P)]),
     "cz_destroy": (None, [_P]),

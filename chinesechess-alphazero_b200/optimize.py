@@ -1,13 +1,21 @@
 """`worker.optimize` drop-in (reference: cchess_alphazero/worker/optimize.py:37-225): learn from the play-data files.
 
 `start(config)` and `OptimizeWorker(config)` keep the reference's method names and control flow: take the play-data
-files in batches of `load_step` (`load_data_steps` where the config has no `load_step`), expand them into training
-tensors (`records.expanding_data`, on the rules kernels), run `epoch_to_checkpoint` epochs of Keras-`fit`-equivalent
-training, save the best model, move the used files to `data/trained/`, and when the files run out save the next
-generation.  The reference compiles a Keras model and calls `fit`; here `compile_model` builds a `train.Trainer`
-(cz_train_step: CUDA forward, backward and SGD-momentum update) and `fit` restates Keras 2.0.8's loop: the last 2 % of
-the samples (before shuffling) validate, the training indices are reshuffled every epoch with numpy's global RNG, the
-final partial batch is kept, lr is constant within one call, and the validation loss is computed in inference mode.
+files in batches of `load_step` (`load_data_steps` where the config has no `load_step`), load them, run
+`epoch_to_checkpoint` epochs of Keras-`fit`-equivalent training, save the best model, move the used files to
+`data/trained/`, and when the files run out save the next generation.  The reference compiles a Keras model and calls
+`fit`; here `compile_model` builds a `train.Trainer` (cz_train_step: CUDA forward, backward and SGD-momentum update) and
+`fit` restates Keras 2.0.8's loop: the last 2 % of the samples (before shuffling) validate, the training indices are
+reshuffled every epoch with numpy's global RNG, the final partial batch is kept, lr is constant within one call, and the
+validation loss is computed in inference mode.
+
+With the built-in trainer the play data stays on the GPU: `fill_queue` packs the files' moves on the host and replays
+every game it loaded in one `cz_play_replay` launch (`records.replay_play_games`) into an `sl_data.SlDataset` of
+104 bytes per position (board, label, value, ply in game), and `fit` expands each batch on the device, 14 or 28 planes.
+The reference's host arrays take 13 388 bytes per position (18 428 with history planes).  With an injected
+`trainer_factory` the files are expanded on the host (`records.expanding_data`) and every batch is numpy.  Both paths
+load the same files in the same order, stop at the same `dataset_size`, draw the same random numbers and hand the
+trainer the same values.
 """
 import os
 import shutil
@@ -19,7 +27,8 @@ from types import SimpleNamespace
 import numpy as np
 
 from .model import CChessModel
-from .records import expanding_data, get_game_data_filenames, read_game_data_from_file
+from .records import (PlayGames, check_labels, expanding_data, get_game_data_filenames, load_play_file,
+                      read_game_data_from_file, replay_play_games, split_games)
 
 logger = getLogger(__name__)
 
@@ -54,12 +63,7 @@ def load_data_from_file(filename, env, use_history=False):
         return None
     if data is None:
         return None
-    games = [[]]
-    for item in data:                     # a file holds nb_game_in_file games back to back: [state, moves..., state, moves...]
-        if isinstance(item, str) and games[-1]:
-            games.append([])
-        games[-1].append(item)
-    out = [expanding_data(g, env, use_history) for g in games if len(g) > 1]
+    out = [expanding_data(g, env, use_history) for g in split_games(data) if len(g) > 1]
     if not out:
         return None
     return tuple(np.concatenate([o[i] for o in out]) for i in range(3))
@@ -78,15 +82,22 @@ def make_batches(size, batch_size):
 
 
 class OptimizeWorker:
-    def __init__(self, config, env=None, trainer_factory=None, device=None):
-        """env: StaticEnv for expanding records (default: the CUDA rules kernels); trainer_factory(model, batch_size, device)
+    def __init__(self, config, env=None, trainer_factory=None, device=None, dataset=None):
+        """env: StaticEnv for replaying records (default: the CUDA rules kernels); trainer_factory(model, batch_size, device)
         builds the object whose step(planes, policy, value, lr) / validation_loss(...) / export() train (default
-        train.Trainer)."""
+        train.Trainer).  dataset: "device" keeps the positions on env's device and hands `step` device tensors, "host"
+        expands them into numpy arrays; the default is "device" with the built-in trainer and "host" with a
+        trainer_factory."""
+        if dataset is None:
+            dataset = "device" if trainer_factory is None else "host"
+        if dataset not in ("device", "host"):
+            raise ValueError(f"dataset must be 'device' or 'host', not {dataset!r}")
+        self.on_device = dataset == "device"
         self.config = config
         self.model = None
         self.loaded_filenames = set()
         self.loaded_data = deque(maxlen=self.config.trainer.dataset_size)
-        self.dataset = deque(), deque(), deque()
+        self.clear_dataset()
         self.filenames = []
         self.opt = None
         self.count = 0
@@ -134,19 +145,23 @@ class OptimizeWorker:
             shuffle(self.filenames)
             self.fill_queue()
             self.update_learning_rate(total_steps)
-            if len(self.dataset[0]) > tc.batch_size:
+            if self.loaded_count() > tc.batch_size:
                 steps = self.train_epoch(tc.epoch_to_checkpoint)
                 total_steps += steps
                 self.save_current_model(send=False)
                 self.update_learning_rate(total_steps)
                 self.count += 1
-                self.dataset = deque(), deque(), deque()
+                self.clear_dataset()
                 self.backup_play_data(files)
         return total_steps
 
     def train_epoch(self, epochs):
         """optimize.py:102-121."""
         tc = self.config.trainer
+        if self.on_device:
+            data = self.collect_all_loaded_data()
+            self.fit_dataset(data, tc.batch_size, epochs)
+            return (len(data) // tc.batch_size) * epochs
         state_ary, policy_ary, value_ary = self.collect_all_loaded_data()
         self.fit(state_ary, policy_ary, value_ary, tc.batch_size, epochs)
         return (state_ary.shape[0] // tc.batch_size) * epochs
@@ -168,6 +183,28 @@ class OptimizeWorker:
             logger.info(f"epoch {epoch + 1}/{epochs}: {rec}")
             self.history.append(rec)
 
+    def fit_dataset(self, data, batch_size, epochs, validation=0.02):
+        """`fit` on the device dataset: the same split, shuffles and batches, each batch expanded on the device
+        (SlDataset.batch); the validation batch is built once, its targets as numpy like `fit` hands them."""
+        env, history = self._env(), self.use_history()
+        train_idx, val_idx = validation_split(len(data), validation)
+        val = None
+        if len(val_idx):
+            p, pol, v = data.batch(env, val_idx, history)
+            val = (p, pol.cpu().numpy(), v.cpu().numpy())
+        lr = self.opt.lr
+        for epoch in range(epochs):
+            order = train_idx.copy()
+            np.random.shuffle(order)
+            losses = []
+            for a, b in make_batches(len(order), batch_size):
+                losses.append(self.trainer.step(*data.batch(env, order[a:b], history), lr))
+            rec = {"epoch": epoch, "lr": lr, "loss": float(np.mean([l[0] for l in losses])) if losses else None}
+            if val is not None:
+                rec["val_loss"] = self.trainer.validation_loss(*val)[0]
+            logger.info(f"epoch {epoch + 1}/{epochs}: {rec}")
+            self.history.append(rec)
+
     def compile_model(self):
         """optimize.py:129-136: SGD(lr=0.02, momentum) on the two losses with config.trainer.loss_weights."""
         self.opt = SimpleNamespace(lr=0.02, momentum=self.config.trainer.momentum)
@@ -183,16 +220,46 @@ class OptimizeWorker:
             self.opt.lr = lr
             logger.debug(f"total step={total_steps}, set learning rate to {lr}")
 
+    def use_history(self):
+        return bool(getattr(getattr(self.config, "opts", None), "has_history", False))
+
+    def loaded_count(self):
+        if self.on_device:
+            return 0 if self.dataset is None else len(self.dataset)
+        return len(self.dataset[0])
+
+    def clear_dataset(self):
+        self.dataset = None if self.on_device else (deque(), deque(), deque())
+
     def fill_queue(self):
-        """optimize.py:150-170, sequential: files popped from the end of the shuffled list until dataset_size samples."""
-        use_history = bool(getattr(getattr(self.config, "opts", None), "has_history", False))
-        while self.filenames and len(self.dataset[0]) < self.config.trainer.dataset_size:
-            t = load_data_from_file(self.filenames.pop(), self._env(), use_history)
+        """optimize.py:150-170, sequential: files popped from the end of the shuffled list until dataset_size samples.
+        On the device path the files are read, packed and label-checked one by one (the same stopping test, counting
+        the positions they hold, and a bad file raising where the host path raises) and then replayed together in one
+        launch."""
+        size = self.config.trainer.dataset_size
+        if self.on_device:
+            env = self._env()
+            parts, pending = [], self.loaded_count()
+            while self.filenames and pending < size:
+                games = load_play_file(self.filenames.pop())
+                if games is not None:
+                    check_labels(games, env.label_lut)
+                    parts.append(games)
+                    pending += len(games)
+            if parts:
+                chunk = replay_play_games(env.lib, env.device, PlayGames.concat(parts), env.label_lut)
+                self.dataset = chunk if self.dataset is None else self.dataset.extend(chunk)
+            return
+        while self.filenames and len(self.dataset[0]) < size:
+            t = load_data_from_file(self.filenames.pop(), self._env(), self.use_history())
             if t is not None:
                 for x, y in zip(self.dataset, t):
                     x.extend(y)
 
     def collect_all_loaded_data(self):
+        """Host path: (planes, policy, value) numpy arrays.  Device path: the SlDataset."""
+        if self.on_device:
+            return self.dataset
         state_ary, policy_ary, value_ary = self.dataset
         return (np.asarray(state_ary, dtype=np.float32), np.asarray(policy_ary, dtype=np.float32),
                 np.asarray(value_ary, dtype=np.float32))

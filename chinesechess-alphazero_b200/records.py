@@ -4,6 +4,7 @@ Record format of the reference (worker/self_play.py:202-208 -> lib/data_helper.p
 `[init_state, [move, value], [move, -value], ...]` with `value` the result from red's view for the first entry and
 alternating sign after it; moves are the 4-digit strings in the mover's own frame.
 """
+import ctypes as C
 import json
 import os
 from datetime import datetime, timedelta, timezone
@@ -13,6 +14,8 @@ import torch
 
 from .env import INIT_STATE, state_to_board
 from .lib import BOARD_STRIDE, MAX_MOVES
+
+CZ_PLAY_OK, CZ_PLAY_FAILED = 0, 1          # cz_play_replay's per-game status
 
 
 def record_to_play_data(rec, init_state=INIT_STATE):
@@ -132,6 +135,139 @@ def get_game_data_filenames(rc):
 def read_game_data_from_file(path):
     with open(path, "rt") as f:
         return json.load(f)
+
+
+def split_games(data):
+    """A play-data file's list -> its games: a file holds nb_game_in_file games back to back, [state, moves..., state,
+    moves...], and every state string after the first item starts a new one."""
+    games = [[]]
+    for item in data:
+        if isinstance(item, str) and games[-1]:
+            games.append([])
+        games[-1].append(item)
+    return games
+
+
+def _move_ok(m):
+    return isinstance(m, str) and len(m) == 4 and all(c in "0123456789" for c in m) and m[0] != "9" and m[2] != "9"
+
+
+def move_codes(moves, source=""):
+    """Moves "x0y0x1y1" (mover's frame) -> uint16 (from << 8) | to with squares y*9+x, in one numpy pass.  A move that is
+    not four ASCII digits or names a square off the board (x = 9) raises ValueError naming `source` and the move."""
+    if not len(moves):
+        return np.zeros(0, np.uint16)
+    try:
+        a = np.asarray(moves)
+        ok = a.ndim == 1 and a.dtype == np.dtype("<U4") and bool((np.char.str_len(a) == 4).all())
+        d = a.astype("S4").view(np.uint8).reshape(-1, 4).astype(np.int32) - 48 if ok else None
+    except (ValueError, TypeError, UnicodeEncodeError):
+        ok = False
+    if ok:
+        ok = bool(((d >= 0) & (d <= 9)).all() and (d[:, 0] <= 8).all() and (d[:, 2] <= 8).all())
+    if not ok:
+        bad = next(m for m in moves if not _move_ok(m))
+        raise ValueError(f"{source}: move {bad!r} is not four digits x0y0x1y1 naming two squares of the board")
+    return (((d[:, 1] * 9 + d[:, 0]) << 8) | (d[:, 3] * 9 + d[:, 2])).astype(np.uint16)
+
+
+class PlayGames:
+    """Games of play-data records packed for cz_play_replay: start boards u8 [n][96], plies per game, move codes u16 [P],
+    values f32 [P]."""
+
+    def __init__(self, boards, counts, codes, values):
+        self.boards, self.counts, self.codes, self.values = boards, counts, codes, values
+
+    def __len__(self):
+        return len(self.codes)
+
+    @staticmethod
+    def concat(parts):
+        return PlayGames(*(np.concatenate([getattr(p, k) for p in parts]) for k in ("boards", "counts", "codes", "values")))
+
+
+def pack_play_games(games, source=""):
+    """Games `[init_state, [move, value], ...]` with at least one move -> PlayGames: state_to_board once per game, the
+    moves in one numpy pass (move_codes) and the values as np.asarray(..., float32), as expanding_data rounds them.
+    Raises ValueError, naming `source`, for a game that does not start with a state or a malformed move."""
+    from itertools import chain
+    from operator import itemgetter
+    if any(not isinstance(g[0], str) for g in games):
+        raise ValueError(f"{source}: a game does not start with a state string")
+    boards = np.stack([state_to_board(g[0]) for g in games])
+    counts = np.array([len(g) - 1 for g in games], np.int64)
+    items = list(chain.from_iterable(g[1:] for g in games))
+    codes = move_codes(list(map(itemgetter(0), items)), source)
+    values = np.asarray(list(map(itemgetter(1), items)), dtype=np.float32)
+    return PlayGames(boards, counts, codes, values)
+
+
+def load_play_file(filename):
+    """optimize.load_data_from_file without the expansion: read, split, drop games without moves, pack.  An unreadable
+    file is deleted (optimize.py:223-232); None when the file holds no game with a move."""
+    import logging
+    try:
+        data = read_game_data_from_file(filename)
+    except Exception as e:
+        logging.getLogger(__name__).error(f"Error when loading data {e}")
+        os.remove(filename)
+        return None
+    if data is None:
+        return None
+    games = [g for g in split_games(data) if len(g) > 1]
+    return pack_play_games(games, filename) if games else None
+
+
+def check_labels(games, lut):
+    """expanding_data's label check on PlayGames, on the host: the first move without an action label raises its
+    ValueError.  OptimizeWorker runs it on every file as it loads, so a bad file stops the load where the host path
+    stops it."""
+    from .env import u16_to_move
+    codes = games.codes.astype(np.int64)
+    bad = np.flatnonzero(np.asarray(lut)[(codes >> 8) * 90 + (codes & 0xFF)] < 0)
+    if len(bad):
+        raise ValueError(f"move {u16_to_move(int(games.codes[bad[0]]))} is not an action label")
+
+
+def play_replay(lib, device, games, lut, stream=None):
+    """One cz_play_replay launch over PlayGames -> (boards u8 [P][96], labels i16 [P] on `device`, status np.int32 [n],
+    offsets np.int64 [n + 1])."""
+    device = torch.device(device)
+    n, total = len(games.counts), len(games.codes)
+    offsets = np.zeros(n + 1, np.int64)
+    np.cumsum(games.counts, out=offsets[1:])
+
+    def dev(a):
+        return torch.from_numpy(np.ascontiguousarray(a)).to(device)
+
+    t_init, t_off = dev(games.boards.astype(np.uint8)), dev(offsets.astype(np.int32))
+    t_moves, t_lut = dev(games.codes.view(np.int16)), dev(np.asarray(lut, np.int16))
+    boards = torch.zeros((max(total, 1), BOARD_STRIDE), dtype=torch.uint8, device=device)
+    labels = torch.full((max(total, 1),), -1, dtype=torch.int16, device=device)
+    status = torch.zeros(max(n, 1), dtype=torch.int32, device=device)
+    if stream is None:
+        stream = C.c_void_p(torch.cuda.current_stream(device).cuda_stream) if lib.is_cuda else C.c_void_p(0)
+    ptr = [C.c_void_p(t.data_ptr()) for t in (t_init, t_off, t_moves, t_lut, boards, labels, status)]
+    lib.call("cz_play_replay", *ptr[:3], n, *ptr[3:], stream)
+    return boards[:total], labels[:total], status[:n].cpu().numpy(), offsets
+
+
+def replay_play_games(lib, device, games, lut, stream=None):
+    """PlayGames -> sl_data.SlDataset with the ply column, in one cz_play_replay launch: per ply the mover-relative board
+    before the move, its label, the record's value and the ply's index in its game.  A game with a move that has no
+    label raises expanding_data's ValueError (the first such game, and its first such move)."""
+    from .env import u16_to_move
+    from .sl_data import SlDataset
+    boards, labels, status, offsets = play_replay(lib, device, games, lut, stream)
+    failed = np.flatnonzero(status != CZ_PLAY_OK)
+    if len(failed):
+        g = int(failed[0])
+        o = int(offsets[g]) + int(np.flatnonzero(labels[offsets[g]:offsets[g + 1]].cpu().numpy() < 0)[0])
+        raise ValueError(f"move {u16_to_move(int(games.codes[o]))} is not an action label")
+    ply = np.arange(len(games), dtype=np.int64) - np.repeat(offsets[:-1], games.counts)
+    device = boards.device
+    return SlDataset(boards, labels, torch.from_numpy(games.values).to(device),
+                     torch.from_numpy(np.minimum(ply, 32767).astype(np.int16)).to(device))
 
 
 def expanding_data(data, env, use_history=False):

@@ -5,7 +5,8 @@ four onegreen digits, with the side list the ply belongs to).  `replay()` walks 
 (`cz_sl_replay`, csrc/cz_replay.cu: one warp per game) and leaves the observation before every ply and its label in device
 tensors.  `build_dataset()` keeps the records `load_game` appends, in its order, and computes their values with numpy.
 A position then costs 96 + 2 + 4 bytes on the device instead of the 14x10x9 float32 planes and 2086-wide float32 policy
-row (13 388 bytes) of the reference's host arrays; `SlDataset.batch()` expands a batch on the device.
+row (13 388 bytes) of the reference's host arrays; `SlDataset.batch()` expands a batch on the device.  The same dataset
+holds OptimizeWorker's self-play records (records.replay_play_games) with a fourth column, the ply in the game.
 """
 import ctypes as C
 import csv
@@ -201,31 +202,47 @@ def record_order(labels, sides, o0, o1):
 
 
 class SlDataset:
-    """boards u8 [N][96], labels i16 [N], values f32 [N] on one device."""
+    """boards u8 [N][96], labels i16 [N], values f32 [N] on one device, and optionally ply i16 [N]: the position's ply in
+    its game (saturating at 32767), for datasets whose games are stored in consecutive rows (self-play records,
+    records.replay_play_games); it lets `batch` build the 28 history planes.  104 bytes per position with it."""
 
-    def __init__(self, boards, labels, values):
-        self.boards, self.labels, self.values = boards, labels, values
+    def __init__(self, boards, labels, values, ply=None):
+        self.boards, self.labels, self.values, self.ply = boards, labels, values, ply
 
     def __len__(self):
         return int(self.boards.shape[0])
 
     @staticmethod
-    def empty(device):
+    def empty(device, with_ply=False):
         return SlDataset(torch.zeros((0, BOARD_STRIDE), dtype=torch.uint8, device=device),
-                         torch.zeros(0, dtype=torch.int16, device=device), torch.zeros(0, dtype=torch.float32, device=device))
+                         torch.zeros(0, dtype=torch.int16, device=device), torch.zeros(0, dtype=torch.float32, device=device),
+                         torch.zeros(0, dtype=torch.int16, device=device) if with_ply else None)
 
     def extend(self, other):
         if other is None or not len(other):
             return self
+        if (self.ply is None) != (other.ply is None):
+            raise ValueError("cannot join a dataset with a ply column and one without")
         return SlDataset(torch.cat([self.boards, other.boards]), torch.cat([self.labels, other.labels]),
-                         torch.cat([self.values, other.values]))
+                         torch.cat([self.values, other.values]),
+                         None if self.ply is None else torch.cat([self.ply, other.ply]))
 
-    def batch(self, env, idx):
+    def batch(self, env, idx, history=False):
         """Training tensors of samples idx (host int array): boards gathered on the device, planes by
-        cz_env_encode_planes, the one-hot policy scattered into a zeroed [B][2086] tensor."""
+        cz_env_encode_planes, the one-hot policy scattered into a zeroed [B][2086] tensor.  history=True: 28 planes,
+        planes 14-27 of a sample those of row idx - 2 (the same game's position two plies earlier) where its ply is >= 2,
+        zero otherwise (an empty board encodes to zero planes) — records.expanding_data(..., use_history=True)."""
         ids = torch.from_numpy(np.ascontiguousarray(idx, np.int64)).to(self.boards.device)
-        boards = self.boards.index_select(0, ids).contiguous()
-        planes = env.planes_batch(boards)
+        boards = self.boards.index_select(0, ids)
+        if history:
+            if self.ply is None:
+                raise ValueError("28-plane batches need the dataset's ply column")
+            earlier = self.boards.index_select(0, (ids - 2).clamp_min(0))
+            earlier = torch.where((self.ply.index_select(0, ids) >= 2).unsqueeze(1), earlier, torch.zeros_like(earlier))
+            both = env.planes_batch(torch.cat([boards, earlier]))
+            planes = torch.cat([both[:len(ids)], both[len(ids):]], dim=1)
+        else:
+            planes = env.planes_batch(boards.contiguous())
         policy = torch.zeros((len(ids), N_LABELS), dtype=torch.float32, device=self.boards.device)
         policy.scatter_(1, self.labels.index_select(0, ids).long().unsqueeze(1), 1.0)
         return planes, policy, self.values.index_select(0, ids)

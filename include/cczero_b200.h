@@ -90,6 +90,21 @@ int cz_sl_replay(const uint8_t* init_boards_dev, const int32_t* ply_offsets_dev,
                  int16_t* labels_out_dev, int32_t* game_out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Self-play records — worker/optimize.py expanding_data :234-281 on the files worker/self_play.py :202-208 writes, one
+ * warp per game
+ * ---------------------------------------------------------------------------------------- */
+enum { CZ_PLAY_OK = 0, CZ_PLAY_FAILED = 1 };   /* FAILED: a ply whose move has no action label (the reference raises) */
+/* Replays n games of the reference's record format: an initial state, then moves "x0y0x1y1" in the mover's own frame.
+ * init_boards_dev [n][96]: the initial state in engine layout (env.state_to_board).  ply_offsets_dev [n + 1]: game g owns
+ * plies [off[g], off[g+1]).  moves_dev [P]: (from << 8) | to, squares y*9+x of the mover's frame.  lut_dev [90*90]:
+ * cz_action_labels' table.  Each ply is senv.step (step_flip), applied unchecked.  Outputs per ply: boards_out_dev [P][96]
+ * the mover-relative board before the move, labels_out_dev [P] the move's label or -1.  status_out_dev [n]: CZ_PLAY_OK,
+ * or CZ_PLAY_FAILED at the first ply without a label (that ply's board and -1 are written, later plies are not). */
+int cz_play_replay(const uint8_t* init_boards_dev, const int32_t* ply_offsets_dev, const uint16_t* moves_dev, int n,
+                   const int16_t* lut_dev, uint8_t* boards_out_dev, int16_t* labels_out_dev, int32_t* status_out_dev,
+                   void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Search engine — agent/player.py (CChessPlayer) for many concurrent games
  * ---------------------------------------------------------------------------------------- */
 typedef struct cz_engine cz_engine;
