@@ -238,9 +238,49 @@ CZ_KERNEL(k_play_replay)(const uint8_t* init, const int32_t* offs, const uint16_
   if (czs::lane() == 0) status_out[g] = status;
 }
 
+// Training targets of visit-recorded plies (cz_visit_targets), one warp per row: target[l_i] = float32(n_i / sum n) with
+// the sum in integers and the division in float64, i.e. numpy's `policy /= np.sum(policy)` on calc_policy's float64
+// counts (player.py:375-406) followed by np.asarray(..., float32).  A row without pairs is the one-hot of its move.
+CZ_KERNEL(k_visit_targets)(const int64_t* offs, const uint16_t* labels, const uint32_t* counts, const int16_t* move_labels,
+                           const int64_t* ids, int n, float* out) {
+  const int r = czs::block_idx() * czs::warps_per_block() + czs::warp_in_block();
+  if (r >= n) return;
+  const int64_t id = ids[r], o0 = offs[id], o1 = offs[id + 1];
+  float* row = out + (size_t)r * N_LABELS;
+  for (int k = czs::lane(); k < N_LABELS; k += 32) row[k] = 0.f;
+  unsigned long long sum = 0;
+  for (int64_t o = o0 + czs::lane(); o < o1; o += 32) sum += counts[o];
+  for (int m = 16; m; m >>= 1) sum += czs::shfl_xor(sum, m);
+  czs::syncwarp();
+  if (o0 == o1) {
+    if (czs::lane() == 0) row[move_labels[id]] = 1.f;
+    return;
+  }
+#if defined(CZ_EMUL)
+  const double den = (double)sum;
+  for (int64_t o = o0 + czs::lane(); o < o1; o += 32) row[labels[o]] = (float)((double)counts[o] / den);
+#else
+  const double den = __ull2double_rn(sum);
+  for (int64_t o = o0 + czs::lane(); o < o1; o += 32) row[labels[o]] = __double2float_rn(__ddiv_rn((double)counts[o], den));
+#endif
+}
+
 }  // namespace
 
 extern "C" {
+
+int cz_visit_targets(const int64_t* offsets, const uint16_t* labels, const uint32_t* counts, const int16_t* move_labels,
+                     const int64_t* ids, int n, float* out, void* stream) {
+  if (n < 0) return cz_fail(CZ_ERR_ARG, "cz_visit_targets: bad n");
+  if (n == 0) return CZ_OK;
+  if (!offsets || !move_labels || !ids || !out) return cz_fail(CZ_ERR_ARG, "cz_visit_targets: null argument");
+  CZ_LAUNCH(k_visit_targets, (n + kWarpsPerBlock - 1) / kWarpsPerBlock, kWarpsPerBlock, 0, (cz_stream_t)stream, offsets, labels,
+            counts, move_labels, ids, n, out);
+  const char* msg;
+  const int e = czrt_last_error(&msg);
+  if (e) return cz_fail(CZ_ERR_CUDA, "cz_visit_targets: %s", msg);
+  return CZ_OK;
+}
 
 int cz_play_replay(const uint8_t* init_boards, const int32_t* ply_offsets, const uint16_t* moves, int n, const int16_t* lut,
                    uint8_t* boards_out, int16_t* labels_out, int32_t* status_out, void* stream) {

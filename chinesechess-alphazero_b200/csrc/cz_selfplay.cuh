@@ -27,6 +27,50 @@ inline void selfplay_carve(SelfplayDev& sp, CarverT& cv, const CfgT& c) {
   sp.enable_resign_rate = c.enable_resign_rate;
 }
 
+// cz_config.record_visits, carved after everything else so that no other buffer moves.  Staging holds the worst case of a
+// game (every ply with MAX_MOVES visited edges), the heap that of a full ring, so the heap cannot overflow while the ring
+// has a slot.  The heap side is one block: [pairs used u64][first pair per record i64 x rec_cap][pairs per ply u8 x
+// rec_cap x hist_stride, padded to 8][pairs (label, N) u32 x 2].
+inline size_t visits_pairs_cap(const SelfplayDev& sp) { return (size_t)sp.rec_cap * sp.hist_stride * MAX_MOVES; }
+inline size_t visits_cnt_off(const SelfplayDev& sp) { return 8 + 8 * (size_t)sp.rec_cap; }
+inline size_t visits_heap_off(const SelfplayDev& sp) { return (visits_cnt_off(sp) + (size_t)sp.rec_cap * sp.hist_stride + 7) & ~(size_t)7; }
+inline size_t visits_block_bytes(const SelfplayDev& sp) { return visits_heap_off(sp) + 8 * visits_pairs_cap(sp); }
+
+template <class CarverT, class CfgT>
+inline void visits_carve(SelfplayDev& sp, CarverT& cv, const CfgT& c) {
+  sp.record_visits = c.record_visits ? 1 : 0;
+  if (!sp.record_visits) return;
+  const size_t G = c.n_games, S = sp.hist_stride;
+  sp.vis_lab = cv.template take<uint16_t>(G * S * MAX_MOVES); sp.vis_n = cv.template take<uint32_t>(G * S * MAX_MOVES);
+  sp.vis_ply = cv.template take<uint8_t>(G * S); sp.vis_cursor = cv.template take<int32_t>(G);
+  uint8_t* blk = cv.template take<uint8_t>(visits_block_bytes(sp));
+  sp.vis_used = reinterpret_cast<unsigned long long*>(blk);
+  sp.rec_vis_off = reinterpret_cast<int64_t*>(blk ? blk + 8 : nullptr);
+  sp.rec_vis_cnt = blk ? blk + visits_cnt_off(sp) : nullptr;
+  sp.vis_heap = reinterpret_cast<uint32_t*>(blk ? blk + visits_heap_off(sp) : nullptr);
+}
+
+// The root's (label, N) pairs of ply `ply` appended to the game's staging, in ascending label order: every edge with
+// N > 0, which excludes the no_act moves (calc_policy zeroes them, player.py:381-383).  Only reads the search's state.
+CZ_D void record_root_visits(const SelfplayDev& sp, int g, int ply, const int nv[4], const int lab[4], int L) {
+  int key[4], rank[4];
+  for (int c = 0; c < 4; ++c) { key[c] = nv[c] > 0 && lab[c] >= 0 ? lab[c] : 0x7fffffff; rank[c] = 0; }
+  for (int j = 0; j < L; ++j) {                     // all lanes walk the same j: broadcast via shfl
+    const int oc = j >> 5;
+    const int ok = czs::shfl(oc == 0 ? key[0] : oc == 1 ? key[1] : oc == 2 ? key[2] : key[3], j & 31);
+    for (int c = 0; c < 4; ++c) rank[c] += ok < key[c] ? 1 : 0;
+  }
+  int kept = 0;
+  for (int c = 0; c < 4; ++c) kept += key[c] != 0x7fffffff ? 1 : 0;
+  kept = czs::warp_sum(kept);
+  const size_t base = (size_t)g * sp.hist_stride * MAX_MOVES + sp.vis_cursor[g];
+  for (int c = 0; c < 4; ++c)
+    if (key[c] != 0x7fffffff) { sp.vis_lab[base + rank[c]] = (uint16_t)key[c]; sp.vis_n[base + rank[c]] = (uint32_t)nv[c]; }
+  czs::syncwarp();
+  if (czs::lane() == 0) { sp.vis_ply[(size_t)g * sp.hist_stride + ply] = (uint8_t)kept; sp.vis_cursor[g] += kept; }
+  czs::syncwarp();
+}
+
 // (Re)start the game in slot g at the position currently in root_board: fresh history, counters and
 // the per-game resign lottery (`random() > enable_resign_rate`, self_play.py:102-105).
 CZ_D void selfplay_start_game(const EngineDev& E, int g, uint8_t* board_smem) {
@@ -39,6 +83,7 @@ CZ_D void selfplay_start_game(const EngineDev& E, int g, uint8_t* board_smem) {
     Rng r; r.init(E.seed, E.rank, (uint32_t)g, 3u, (uint32_t)idx);
     sp.enable_resign[g] = r.uniform() > sp.enable_resign_rate ? 1 : 0;
     sp.turns[g] = 0; sp.no_eat[g] = 0;
+    if (sp.record_visits) sp.vis_cursor[g] = 0;
     // evaluator.py:153-154: `playouts = randint(8, 12) * 100` once per game; both player slots of a game draw the same value
     int sg = 0;
     if (E.arena && sp.playouts_lo > 0 && sp.playouts_hi >= sp.playouts_lo) {
@@ -208,6 +253,7 @@ CZ_D void game_play(const EngineDev& E, int g, const uint8_t* init_board, TreeSm
       chosen = 0;
     }
     const move_t mv = E.edge_move[eo + chosen];
+    if (sp.record_visits) record_root_visits(sp, g, turns0, nv, lab, L);
     // ---- play it (self_play.py:132-147)
     copy_board(E.root_board + (size_t)g * BOARD_STRIDE, sm->board);
     const bool no_eat = step_flip(sm->board, mv, sm->board);
@@ -251,7 +297,10 @@ CZ_D void game_play(const EngineDev& E, int g, const uint8_t* init_board, TreeSm
       }
     }
     if (over && final_from_to >= 0) {                // the king capture is appended to the record (:177-184)
-      if (czs::lane() == 0) sp.hist_move[(size_t)g * sp.hist_stride + turns] = (uint16_t)final_from_to;
+      if (czs::lane() == 0) {
+        sp.hist_move[(size_t)g * sp.hist_stride + turns] = (uint16_t)final_from_to;
+        if (sp.record_visits) sp.vis_ply[(size_t)g * sp.hist_stride + turns] = 0;     // never searched
+      }
       ++turns;
       value = -value;
     }
@@ -296,6 +345,25 @@ CZ_D void game_play(const EngineDev& E, int g, const uint8_t* init_board, TreeSm
     }
     for (int i = czs::lane(); i < turns; i += 32)
       sp.rec_moves[(size_t)slot * sp.hist_stride + i] = sp.hist_move[(size_t)g * sp.hist_stride + i];
+    if (sp.record_visits) {                          // the staged pairs into the heap, claimed like the ring slot
+      const int np = sp.vis_cursor[g];
+      unsigned long long off = 0;
+      if (czs::lane() == 0) {
+#if defined(CZ_EMUL)
+        off = sp.vis_used[0]; sp.vis_used[0] = off + (unsigned long long)np;
+#else
+        off = atomicAdd(sp.vis_used, (unsigned long long)np);
+#endif
+        sp.rec_vis_off[slot] = (int64_t)off;
+      }
+      off = czs::shfl(off, 0);
+      const size_t src = (size_t)g * sp.hist_stride;
+      for (int i = czs::lane(); i < turns; i += 32) sp.rec_vis_cnt[(size_t)slot * sp.hist_stride + i] = sp.vis_ply[src + i];
+      for (int i = czs::lane(); i < np; i += 32) {
+        sp.vis_heap[2 * (off + i)] = sp.vis_lab[src * MAX_MOVES + i];
+        sp.vis_heap[2 * (off + i) + 1] = sp.vis_n[src * MAX_MOVES + i];
+      }
+    }
   }
   // ---- quota reached: the slot (both player slots of an arena game) retires with an empty tree
   if (sp.game_quota > 0 && game_index_of(E, g, sp.games_started[g] + 1) >= sp.game_quota) {

@@ -37,6 +37,17 @@ struct SelfplayDev {
   uint16_t* rec_moves;     // [rec_cap][hist_stride]
   int32_t* rec_count;      // [1] records in the ring
   int32_t* finished;       // [1] games finished by the last cz_play_move
+  // cz_config.record_visits: every ply's root visit counts (calc_policy's N(s,a), player.py:375-406).  Staging per game
+  // (ascending label order within a ply), copied at game end into a pair heap beside the ring (cz_record_visits_layout)
+  uint16_t* vis_lab;       // [G][hist_stride * MAX_MOVES] staged labels of the game in the slot
+  uint32_t* vis_n;         // [G][hist_stride * MAX_MOVES] staged N
+  uint8_t* vis_ply;        // [G][hist_stride] pairs per ply (0 for an appended final king capture)
+  int32_t* vis_cursor;     // [G] pairs staged so far
+  unsigned long long* vis_used;  // [1] pairs claimed in the heap (bump allocator)
+  int64_t* rec_vis_off;    // [rec_cap] first heap pair of the record
+  uint8_t* rec_vis_cnt;    // [rec_cap][hist_stride] pairs per ply of the record
+  uint32_t* vis_heap;      // [rec_cap * hist_stride * MAX_MOVES][2] (label, N)
+  int32_t record_visits;
   int32_t rec_cap, hist_stride;
   int32_t game_quota, playouts_lo, playouts_hi;
   double enable_resign_rate;

@@ -419,6 +419,7 @@ size_t carve(cz_engine* e, uint8_t* base) {
   } else {
     e->policy_buf = nullptr; e->value_buf = nullptr; e->legal_p = nullptr;
   }
+  visits_carve(d.sp, cv, c);
   return cv.off + 1024;
 }
 
@@ -435,6 +436,8 @@ int check_cfg(const cz_config* c) {
   if (c->game_quota < 0 || c->playouts_lo < 0 || c->playouts_hi < c->playouts_lo)
     return cz_fail(CZ_ERR_ARG, "cz_config: bad game_quota / playouts range");
   if (c->arena && (c->n_games % 2)) return cz_fail(CZ_ERR_ARG, "cz_config: arena mode needs an even number of slots (two per game)");
+  // the arena's records are scored, never trained on (evaluator.py), and its two slots per game would need a shared staging
+  if (c->arena && c->record_visits) return cz_fail(CZ_ERR_ARG, "cz_config: record_visits is for self-play engines, not arena ones");
   return 0;
 }
 

@@ -22,7 +22,8 @@ class Engine:
                  max_nodes_per_game=None, max_edges_per_game=None, max_path=128, noise_mode=1, max_game_length=100,
                  nn_filters=0, nn_blocks=0, nn_value_fc=256, c_puct=1.5, noise_eps=0.15, dirichlet_alpha=0.2,
                  tau_decay_rate=0.9, resign_threshold=-0.98, enable_resign_rate=0.5, min_resign_turn=40, seed=0, rank=0, nn_fp32_skip=None, arena=False,
-                 use_history=False, game_quota=0, playouts=None, nn_policy_channels=0, nn_value_channels=0):
+                 use_history=False, game_quota=0, playouts=None, nn_policy_channels=0, nn_value_channels=0,
+                 record_visits=False):
         self.lib = lib or get_lib()
         if device is None:
             device = 'cuda' if self.lib.is_cuda else 'cpu'
@@ -53,6 +54,8 @@ class Engine:
         cfg.playouts_lo, cfg.playouts_hi = (playouts or (0, 0))   # arena: per-game randint(lo, hi) * 100 simulations per move
         # head widths of the weight file (0 = agent/model.py's 4 policy / 2 value channels; legacy configs: 2 or 32 / 4)
         cfg.nn_policy_channels, cfg.nn_value_channels = int(nn_policy_channels or 0), int(nn_value_channels or 0)
+        cfg.record_visits = 1 if record_visits else 0   # every ply's root visit counts go with the records (drain_records)
+        self.record_visits = bool(record_visits)
         self.use_history = bool(use_history)
         self.in_planes = 28 if use_history else 14
         self.cfg = cfg
@@ -325,18 +328,43 @@ class Engine:
         return a
 
     def drain_records(self, cap=None):
+        """Finished games: dicts n_plies, value_red, game_index, flags, moves.  A record_visits engine adds "visits": per
+        ply the root's (label, n) pairs in ascending label order (labels index ActionLabelsRed, moves in the mover's
+        frame), [] for an appended final king capture."""
         cap = cap or max(64, 2 * self.n_games)
         row = self.cfg.max_plies + 1
         hdr = (CzRecordHdr * cap)()
         moves = np.zeros((cap, row), dtype=np.uint16)
         n = C.c_int32(0)
-        self.lib.call("cz_drain_records", self._h, C.cast(hdr, C.c_void_p), C.c_void_p(moves.ctypes.data), cap, C.byref(n))
+        if self.record_visits:
+            from .records import split_visit_pairs
+            per_ply = np.zeros((cap, row), dtype=np.uint8)
+            ptr, used = C.c_void_p(0), C.c_uint64(0)       # the drained pairs are at most those in the heap
+            self.lib.call("cz_record_visits_buffer", self._h, C.byref(ptr), C.byref(used))
+            pair_cap = (used.value - self.visits_layout()[2]) // 8
+            pairs = np.zeros((pair_cap, 2), dtype=np.uint32)
+            n_pairs = C.c_int64(0)
+            self.lib.call("cz_drain_records_visits", self._h, C.cast(hdr, C.c_void_p), C.c_void_p(moves.ctypes.data),
+                          C.c_void_p(per_ply.ctypes.data), C.c_void_p(pairs.ctypes.data), pair_cap, cap, C.byref(n),
+                          C.byref(n_pairs))
+            visits = split_visit_pairs(per_ply[:n.value], [hdr[i].n_plies for i in range(n.value)], pairs[:n_pairs.value])
+        else:
+            self.lib.call("cz_drain_records", self._h, C.cast(hdr, C.c_void_p), C.c_void_p(moves.ctypes.data), cap, C.byref(n))
         out = []
         for i in range(n.value):
             h = hdr[i]
             out.append({"n_plies": h.n_plies, "value_red": h.value_red, "game_index": h.game_index, "flags": h.flags,
                         "moves": [u16_to_move(v) for v in moves[i, :h.n_plies]]})
+            if self.record_visits:
+                out[-1]["visits"] = visits[i]
         return out
+
+    def visits_layout(self):
+        """cz_record_visits_layout: byte offsets of the per-record first pair, the per-ply pair counts and the pairs inside
+        the visit block, and its size."""
+        a = np.zeros(4, dtype=np.int64)
+        self.lib.call("cz_record_visits_layout", self._h, C.c_void_p(a.ctypes.data))
+        return tuple(int(x) for x in a)
 
     # ---- network
     def set_weights(self, named_tensors, net=0):

@@ -32,7 +32,7 @@ class CzConfig(C.Structure):
         ("min_resign_turn", C.c_int32), ("max_game_length", C.c_int32),
         ("seed", C.c_uint64), ("rank", C.c_int32), ("arena", C.c_int32), ("nn_fp32_skip", C.c_int32), ("use_history", C.c_int32),
         ("game_quota", C.c_int32), ("playouts_lo", C.c_int32), ("playouts_hi", C.c_int32),
-        ("nn_policy_channels", C.c_int32), ("nn_value_channels", C.c_int32), ("reserved0", C.c_int32),
+        ("nn_policy_channels", C.c_int32), ("nn_value_channels", C.c_int32), ("record_visits", C.c_int32),
     ]
 
 
@@ -125,6 +125,10 @@ _SIGS = {
     "cz_clear_records": (C.c_int, [_P]),
     "cz_drain_records": (C.c_int, [_P, _P, _P, C.c_int32, C.POINTER(C.c_int32)]),
     "cz_record_buffer": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]),
+    "cz_drain_records_visits": (C.c_int, [_P, _P, _P, _P, _P, C.c_int64, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int64)]),
+    "cz_record_visits_buffer": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_uint64)]),
+    "cz_record_visits_layout": (C.c_int, [_P, _P]),
+    "cz_visit_targets": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, _P, _P]),
     "cz_nn_set_weights": (C.c_int, [_P, C.POINTER(CzTensorDesc), C.c_int32]),
     "cz_nn_set_weights_net": (C.c_int, [_P, C.c_int32, C.POINTER(CzTensorDesc), C.c_int32]),
     "cz_nn_forward": (C.c_int, [_P, _P, C.c_int32, _P, _P]),

@@ -16,6 +16,11 @@ The reference's host arrays take 13 388 bytes per position (18 428 with history 
 `trainer_factory` the files are expanded on the host (`records.expanding_data`) and every batch is numpy.  Both paths
 load the same files in the same order, stop at the same `dataset_size`, draw the same random numbers and hand the
 trainer the same values.
+
+`policy_target="visits"` trains the policy head on the search's visit distribution where the records carry it
+(self-play with `record_visits`, records.py): target[l] = float32(n_l / sum n), the AlphaZero target calc_policy builds
+(agent/player.py:375-406).  Plies without visits, such as the appended final king capture or older files, keep the
+one-hot of their move.  The default "move" is the reference's one-hot target (optimize.py:248).
 """
 import os
 import shutil
@@ -27,14 +32,14 @@ from types import SimpleNamespace
 import numpy as np
 
 from .model import CChessModel
-from .records import (PlayGames, check_labels, expanding_data, get_game_data_filenames, load_play_file,
+from .records import (PlayGames, check_labels, expanding_data, get_game_data_filenames, load_play_file, pack_visits,
                       read_game_data_from_file, replay_play_games, split_games)
 
 logger = getLogger(__name__)
 
 
-def start(config):
-    return OptimizeWorker(config).start()
+def start(config, policy_target="move"):
+    return OptimizeWorker(config, policy_target=policy_target).start()
 
 
 def load_best_model_weight(model):
@@ -52,9 +57,10 @@ def save_as_next_generation_model(model):
     model.save(rc.next_generation_config_path, rc.next_generation_weight_path)
 
 
-def load_data_from_file(filename, env, use_history=False):
+def load_data_from_file(filename, env, use_history=False, policy_target="move"):
     """optimize.py:223-232: a file that cannot be read is deleted.  Where the reference's expanding_data reads a file as ONE
-    game (and rejects files of several games: the second initial state is not a move), every game of the file is expanded."""
+    game (and rejects files of several games: the second initial state is not a move), every game of the file is expanded.
+    policy_target as in records.expanding_data; malformed visits raise before any game of the file is expanded."""
     try:
         data = read_game_data_from_file(filename)
     except Exception as e:
@@ -63,7 +69,10 @@ def load_data_from_file(filename, env, use_history=False):
         return None
     if data is None:
         return None
-    out = [expanding_data(g, env, use_history) for g in split_games(data) if len(g) > 1]
+    games = [g for g in split_games(data) if len(g) > 1]
+    if policy_target == "visits":
+        pack_visits([it for g in games for it in g[1:]], filename)
+    out = [expanding_data(g, env, use_history, policy_target, filename) for g in games]
     if not out:
         return None
     return tuple(np.concatenate([o[i] for o in out]) for i in range(3))
@@ -82,17 +91,21 @@ def make_batches(size, batch_size):
 
 
 class OptimizeWorker:
-    def __init__(self, config, env=None, trainer_factory=None, device=None, dataset=None):
+    def __init__(self, config, env=None, trainer_factory=None, device=None, dataset=None, policy_target="move"):
         """env: StaticEnv for replaying records (default: the CUDA rules kernels); trainer_factory(model, batch_size, device)
         builds the object whose step(planes, policy, value, lr) / validation_loss(...) / export() train (default
         train.Trainer).  dataset: "device" keeps the positions on env's device and hands `step` device tensors, "host"
         expands them into numpy arrays; the default is "device" with the built-in trainer and "host" with a
-        trainer_factory."""
+        trainer_factory.  policy_target: "move" (one-hot of the played move) or "visits" (the recorded visit
+        distribution where a ply has one)."""
         if dataset is None:
             dataset = "device" if trainer_factory is None else "host"
         if dataset not in ("device", "host"):
             raise ValueError(f"dataset must be 'device' or 'host', not {dataset!r}")
         self.on_device = dataset == "device"
+        if policy_target not in ("move", "visits"):
+            raise ValueError(f"policy_target must be 'move' or 'visits', not {policy_target!r}")
+        self.policy_target = policy_target
         self.config = config
         self.model = None
         self.loaded_filenames = set()
@@ -241,7 +254,7 @@ class OptimizeWorker:
             env = self._env()
             parts, pending = [], self.loaded_count()
             while self.filenames and pending < size:
-                games = load_play_file(self.filenames.pop())
+                games = load_play_file(self.filenames.pop(), self.policy_target == "visits")
                 if games is not None:
                     check_labels(games, env.label_lut)
                     parts.append(games)
@@ -251,7 +264,7 @@ class OptimizeWorker:
                 self.dataset = chunk if self.dataset is None else self.dataset.extend(chunk)
             return
         while self.filenames and len(self.dataset[0]) < size:
-            t = load_data_from_file(self.filenames.pop(), self._env(), self.use_history())
+            t = load_data_from_file(self.filenames.pop(), self._env(), self.use_history(), self.policy_target)
             if t is not None:
                 for x, y in zip(self.dataset, t):
                     x.extend(y)

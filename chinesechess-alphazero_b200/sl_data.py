@@ -204,10 +204,13 @@ def record_order(labels, sides, o0, o1):
 class SlDataset:
     """boards u8 [N][96], labels i16 [N], values f32 [N] on one device, and optionally ply i16 [N]: the position's ply in
     its game (saturating at 32767), for datasets whose games are stored in consecutive rows (self-play records,
-    records.replay_play_games); it lets `batch` build the 28 history planes.  104 bytes per position with it."""
+    records.replay_play_games); it lets `batch` build the 28 history planes.  104 bytes per position with it.
+    visits: optional CSR columns (offsets i64 [N+1], labels [pairs] int16 holding the u16 labels, counts [pairs] int32
+    holding the u32 counts) of records with root visit counts: `batch` then builds the visit-count targets
+    (cz_visit_targets).  8 bytes per position plus 6 per pair."""
 
-    def __init__(self, boards, labels, values, ply=None):
-        self.boards, self.labels, self.values, self.ply = boards, labels, values, ply
+    def __init__(self, boards, labels, values, ply=None, visits=None):
+        self.boards, self.labels, self.values, self.ply, self.visits = boards, labels, values, ply, visits
 
     def __len__(self):
         return int(self.boards.shape[0])
@@ -223,9 +226,15 @@ class SlDataset:
             return self
         if (self.ply is None) != (other.ply is None):
             raise ValueError("cannot join a dataset with a ply column and one without")
+        if (self.visits is None) != (other.visits is None):
+            raise ValueError("cannot join a dataset with visit columns and one without")
+        visits = None
+        if self.visits is not None:
+            (o0, l0, n0), (o1, l1, n1) = self.visits, other.visits
+            visits = (torch.cat([o0, o1[1:] + o0[-1]]), torch.cat([l0, l1]), torch.cat([n0, n1]))
         return SlDataset(torch.cat([self.boards, other.boards]), torch.cat([self.labels, other.labels]),
                          torch.cat([self.values, other.values]),
-                         None if self.ply is None else torch.cat([self.ply, other.ply]))
+                         None if self.ply is None else torch.cat([self.ply, other.ply]), visits)
 
     def batch(self, env, idx, history=False):
         """Training tensors of samples idx (host int array): boards gathered on the device, planes by
@@ -243,9 +252,21 @@ class SlDataset:
             planes = torch.cat([both[:len(ids)], both[len(ids):]], dim=1)
         else:
             planes = env.planes_batch(boards.contiguous())
-        policy = torch.zeros((len(ids), N_LABELS), dtype=torch.float32, device=self.boards.device)
-        policy.scatter_(1, self.labels.index_select(0, ids).long().unsqueeze(1), 1.0)
+        if self.visits is not None:
+            policy = self.visit_targets(env.lib, ids)
+        else:
+            policy = torch.zeros((len(ids), N_LABELS), dtype=torch.float32, device=self.boards.device)
+            policy.scatter_(1, self.labels.index_select(0, ids).long().unsqueeze(1), 1.0)
         return planes, policy, self.values.index_select(0, ids)
+
+    def visit_targets(self, lib, ids):
+        """cz_visit_targets for the rows ids (int64 device tensor): [B][2086] f32, one-hot where a row has no pairs."""
+        off, lab, n = self.visits
+        out = torch.empty((len(ids), N_LABELS), dtype=torch.float32, device=self.boards.device)
+        stream = C.c_void_p(torch.cuda.current_stream(out.device).cuda_stream) if lib.is_cuda else C.c_void_p(0)
+        lib.call("cz_visit_targets", _ptr(off), _ptr(lab), _ptr(n), _ptr(self.labels), _ptr(ids.contiguous()), len(ids),
+                 _ptr(out), stream)
+        return out
 
 
 def build_dataset(rep, red_wins):

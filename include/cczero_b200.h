@@ -103,6 +103,14 @@ enum { CZ_PLAY_OK = 0, CZ_PLAY_FAILED = 1 };   /* FAILED: a ply whose move has n
 int cz_play_replay(const uint8_t* init_boards_dev, const int32_t* ply_offsets_dev, const uint16_t* moves_dev, int n,
                    const int16_t* lut_dev, uint8_t* boards_out_dev, int16_t* labels_out_dev, int32_t* status_out_dev,
                    void* stream);
+/* Policy targets of n positions of a dataset whose plies carry root visit counts (cz_config.record_visits records): the
+ * pairs of position p are offsets_dev[p] .. offsets_dev[p+1]-1 of labels_dev (u16, < 2086) / counts_dev (u32, > 0).
+ * out_dev [n][2086] f32, row r for position ids_dev[r]: target[label] = float32(N / sum N), the sum in integers and the
+ * division in float64 — numpy's `policy /= np.sum(policy)` on calc_policy's float64 counts (agent/player.py:403) then
+ * np.asarray(..., float32).  A position without pairs gets the one-hot of move_labels_dev[p] (the reference's
+ * build_policy(final_move), worker/self_play.py:180).  Stream-ordered. */
+int cz_visit_targets(const int64_t* offsets_dev, const uint16_t* labels_dev, const uint32_t* counts_dev,
+                     const int16_t* move_labels_dev, const int64_t* ids_dev, int n, float* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Search engine — agent/player.py (CChessPlayer) for many concurrent games
@@ -151,7 +159,9 @@ typedef struct cz_config {
   int32_t nn_policy_channels;  /* filters of the policy 1x1 convolution: 0 = 4 (agent/model.py:47); the older shipped configs use 2
                                 * (data/model/model_128f.json, model_256f.json) and 32 (model_128_l1_config.json) */
   int32_t nn_value_channels;   /* filters of the value 1x1 convolution: 0 = 2 (agent/model.py:56); the older configs use 4 */
-  int32_t reserved0;
+  int32_t record_visits;       /* 1: the on-device game loop records every ply's root visit counts, calc_policy's N(s,a) with the
+                                * no_act moves zeroed (agent/player.py:375-406; worker/self_play.py:112,134 keep the policy the
+                                * reference commented out).  Read them with cz_drain_records_visits.  Not with arena */
 } cz_config;
 
 /* Device workspace the caller must provide (a torch.uint8 CUDA tensor). */
@@ -311,8 +321,24 @@ int cz_record_buffer(cz_engine* e, void** dev_ptr, uint64_t* bytes, int32_t* n_r
  * slots per record row, out[2] = byte offset of the move rows inside the buffer (the headers start at 0, 16 bytes each),
  * out[3] = total bytes.  Host-only. */
 int cz_record_layout(cz_engine* e, int64_t* out /* [4] */);
-/* Forget the records in the ring (after a gather shipped them).  Stream-ordered. */
+/* Forget the records in the ring (after a gather shipped them), and their visit pairs.  Stream-ordered. */
 int cz_clear_records(cz_engine* e);
+/* cz_config.record_visits engines: cz_drain_records plus every record's root visit counts, the policy calc_policy builds
+ * (agent/player.py:375-406) that worker/self_play.py:112,134,178-180 keeps commented out.  ply_pairs_host [cap][max_plies+1]
+ * u8: (label, N) pairs per ply, 0 for the appended final king capture (never searched; self_play.py:180 would one-hot it);
+ * pairs_host [pair_cap][2] u32 (label, N): the records' plies in order, each ply's pairs in ascending label order, every
+ * root edge with N > 0 (no_act moves are zeroed, player.py:381-383); labels index ActionLabelsRed in the mover's frame.
+ * *n records, *n_pairs pairs.  Then clears the ring like cz_drain_records (which, on such an engine, drops the pairs).
+ * Synchronises. */
+int cz_drain_records_visits(cz_engine* e, cz_record_hdr* hdr_host, uint16_t* moves_host, uint8_t* ply_pairs_host,
+                            uint32_t* pairs_host, int64_t pair_cap, int32_t cap, int32_t* n, int64_t* n_pairs);
+/* Device-side view of the visit pairs beside the ring (record_visits engines; CZ_ERR_STATE otherwise): *dev_ptr the block,
+ * *used_bytes its prefix that holds every pair of the records in the ring (what a gather ships).  Synchronises. */
+int cz_record_visits_buffer(cz_engine* e, void** dev_ptr, uint64_t* used_bytes);
+/* Layout of that block: bytes 0-7 u64 = pairs used; out[0] = byte offset of the first heap pair per ring slot (i64
+ * [ring capacity]), out[1] = byte offset of the pairs per ply (u8 [ring capacity][uint16 slots per record row, see
+ * cz_record_layout out[1]]), out[2] = byte offset of the pairs (u32 [][2] = label, N), out[3] = total bytes.  Host-only. */
+int cz_record_visits_layout(cz_engine* e, int64_t* out /* [4] */);
 
 /* ------------------------------------------------------------------------------------------
  * Policy + value network — agent/model.py:32-83 behind agent/api.py:37-74
