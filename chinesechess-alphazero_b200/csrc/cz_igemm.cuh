@@ -4,14 +4,10 @@
 // Replaces the Conv2D/BatchNormalization/Add/Activation stack of agent/model.py:68-83 (residual
 // block) and the Dense of :54 (policy_out) that the reference runs through Keras/TF/cuDNN.
 //
-// Activation layouts in HBM (fp16, channels contiguous):
-//   dense  (conv == 2, the production layout): [n_boards*90][C] pixels.  A 3x3 tap (dy,dx) of 128 consecutive output pixels
-//          is ONE im2col-mode TMA load (64 channels x 128 pixels); taps outside the board are zero-filled by the TMA unit and
-//          the 128-pixel column walks across rows and boards.
-//   strip  (conv == 1): [n_boards*11][9][C].  Board b occupies strip rows b*11 .. b*11+9 (network row r = 9 - y), strip row
-//          b*11+10 is an all-zero separator shared as the vertical halo of board b (below) and b+1 (above).  A tap is ONE
-//          tiled TMA box load at coordinates (c0, dx, r0+dy) of 14 strip rows x 9 columns = 126 pixels (rows 126,127 of the
-//          M tile are don't-care: an A row only feeds the same D row).
+// Operand A in HBM (fp16):
+//   conv (conv == 1): activations [n_boards*90][C] pixels, channels contiguous.  A 3x3 tap (dy,dx) of 128 consecutive output
+//          pixels is ONE im2col-mode TMA load (64 channels x 128 pixels); taps outside the board are zero-filled by the TMA
+//          unit and the 128-pixel column walks across rows and boards.
 //   GEMM   (conv == 0): A [M][K] rows, 128 per tile.
 // Tile: M = 128 pixels / rows, N = N_TILE output channels (<= 256), K walks taps x C_in in 64-channel blocks (128-byte
 //   swizzled rows).  Every output element accumulates its K blocks in the same order whatever the tile shape, so results do
@@ -21,7 +17,7 @@
 //   (+bias (+residual) -> ReLU -> fp16 / fp32 -> HBM).  kStages-deep smem ring with full/empty mbarriers; the producer runs
 //   ahead into the next tile while the consumers store the current one.  Persistent: grid <= #SMs, tiles strided over CTAs.
 //   After the role split the producer warpgroup gives its registers to the consumers (setmaxnreg).
-// Staged epilogue (Args::staged: dense conv without a skip stream, fp16 out, M tiles that lie wholly inside the batch): the
+// Staged epilogue (Args::staged: conv without a skip stream, fp16 out, M tiles that lie wholly inside the batch): the
 //   tile leaves in 32-column steps through a small ring of slots per consumer warpgroup.  A slot holds 64 rows x 32 fp16
 //   columns (64-byte rows, SWIZZLE_64B, as the output's tensor map expects); the warpgroup writes a step into a slot and one
 //   thread hands it to a TMA store, so the stores are whole sectors and drain while the next tile's MMAs run.  The arithmetic
@@ -49,15 +45,13 @@ constexpr int kEpiBytes = kEpiSlots * kEpiSlotBytes;
 struct Args {
   int n_taps;        // 9 (3x3 conv) or 1 (plain GEMM)
   int k_chunks;      // C_in / 64
-  int m_tiles;       // ceil(rows / pixels per tile) (an upper bound when n_dev is set)
+  int m_tiles;       // ceil(rows / kTileM): the host's grid bound (an upper bound when n_dev is set)
   int n_tiles;       // ceil(N / N_TILE)
-  int box_w;         // 9 (strip conv) or 1 (GEMM)
-  int box_r;         // 14 (strip conv) or 128 (GEMM): A-box extent along the outer row dimension
-  int rows;          // strip conv: strip rows (n_boards*11); dense conv: pixels; GEMM: M
+  int rows;          // conv: pixels (n_boards*90); GEMM: M
   int n_total;       // B-operand rows per tap (C_out padded to N_TILE multiple)
   int n_valid;       // real number of output columns
   int ldo;           // output leading dimension in elements
-  int conv;          // 1: strip layout, separator rows forced to zero; 2: dense [B*90][C] pixels fed by im2col TMA; 0: GEMM
+  int conv;          // 1: 3x3 conv over [B*90][C] pixels fed by im2col TMA; 0: GEMM
   int relu;
   int out_f32;       // 1: float output (GEMM logits), 0: fp16
   const float* bias; // [n_total] or null
@@ -65,15 +59,14 @@ struct Args {
   const float* residual32; // fp32 skip stream (takes precedence over `residual`) or null
   float* out32;            // optional fp32 copy of the output (the skip stream of the next block) or null
   void* out;
-  uint32_t a_bytes;  // TMA bytes per A box
   // Batch size read on the DEVICE (fixed-shape launches: the host never learns how many leaves a wave produced).  When
   // n_dev != null, rows = *n_dev * rows_per_unit and m_tiles follows; `rows` / `m_tiles` above are then only upper bounds.
   const int* n_dev;
-  int rows_per_unit; // 90 pixels per board (dense conv), 1 (GEMM rows = positions)
+  int rows_per_unit; // 90 pixels per board (conv), 1 (GEMM rows = positions)
   // GEMM mode (out_f32): per output row and N tile the pair {max_j x_j, sum_j exp(x_j - max)} over the tile's valid
   // columns — the softmax is finished by whoever reads the logits (k_softmax / k_legal_priors), never a second full pass
   float2* row_stats; // [rows][n_tiles] or null
-  int staged;        // dense conv, fp16 out, no skip: tmOut is valid, full M tiles take the staged epilogue
+  int staged;        // conv, fp16 out, no skip: tmOut is valid, full M tiles take the staged epilogue
 };
 
 // rows / m-tiles of this launch (device-side batch size)
@@ -116,7 +109,7 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
 
   const int n_kb = a.n_taps * a.k_chunks;
   const int rows = args_rows(a);
-  const int m_tiles = a.conv == 1 ? a.m_tiles : (rows + kTileM - 1) / kTileM;
+  const int m_tiles = (rows + kTileM - 1) / kTileM;
   const int total_tiles = m_tiles * a.n_tiles;
 
   constexpr int kSteps = N_TILE / kEpiCols;                // steps of the staged epilogue per tile
@@ -128,18 +121,18 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
     if (t == 0) {
       wg::prefetch_tmap(&tmA);
       wg::prefetch_tmap(&tmB);
-      // Dense conv with a skip stream: the epilogue reads the tile's skip rows right after the last MMA, when every CTA of the
+      // Conv with a skip stream: the epilogue reads the tile's skip rows right after the last MMA, when every CTA of the
       // wave does the same, so the reads would all miss L2 at once with the tensor cores idle.  Halfway through the tile's
       // main loop the producer prefetches them into L2 instead (rows below args_rows only; at N_TILE = ldo one contiguous
       // range, else one range per row).  Halfway rather than at the tile's first load: the first load is issued while the
       // previous tile's epilogue still has to stream its outputs through L2, which could evict the prefetched lines.
-      const uint8_t* skip = a.conv != 2 ? nullptr : a.residual32 ? reinterpret_cast<const uint8_t*>(a.residual32)
-                                                                 : reinterpret_cast<const uint8_t*>(a.residual);
+      const uint8_t* skip = !a.conv ? nullptr : a.residual32 ? reinterpret_cast<const uint8_t*>(a.residual32)
+                                                               : reinterpret_cast<const uint8_t*>(a.residual);
       const int skip_es = a.residual32 ? 4 : 2;
       uint32_t s = 0, ph = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int m_tile = tile % m_tiles, n_tile = tile / m_tiles;
-        // dense mode: first output pixel of this tile as (image, row, column); im2col walks on from there
+        // conv: first output pixel of this tile as (image, row, column); im2col walks on from there
         const int pix0 = m_tile * kTileM, img0 = pix0 / 90, row0 = (pix0 % 90) / 9, col0 = pix0 % 9;
         for (int tap = 0; tap < a.n_taps; ++tap) {
           const int dy = a.n_taps == 9 ? tap / 3 - 1 : 0;
@@ -156,11 +149,11 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
             wg::mbar_wait(&empty[s], ph ^ 1);
             uint8_t* sA = smem + s * C::kStageBytes;
             uint8_t* sB = sA + kAStageBytes;
-            wg::mbar_expect_tx(&full[s], a.a_bytes + (uint32_t)C::kBStageBytes);
-            if (a.conv == 2)
+            wg::mbar_expect_tx(&full[s], (uint32_t)C::kStageBytes);
+            if (a.conv)
               wg::tma_load_im2col_4d(sA, &tmA, &full[s], kc * kBlockK, col0 - 1, row0 - 1, img0, (uint16_t)(dx + 1), (uint16_t)(dy + 1));
             else
-              wg::tma_load_3d(sA, &tmA, &full[s], kc * kBlockK, dx, m_tile * a.box_r + dy);
+              wg::tma_load_2d(sA, &tmA, &full[s], kc * kBlockK, m_tile * kTileM);
             wg::tma_load_2d(sB, &tmB, &full[s], kc * kBlockK, tap * a.n_total + n_tile * N_TILE);
             if (++s == (uint32_t)S) { s = 0; ph ^= 1; }
           }
@@ -251,19 +244,10 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
       }
       continue;
     }
-    // accumulator row mrow + 8h: global output row, inside the batch, strip separator row (stays zero)
-    auto out_row = [&](int h, long long& grow, bool& valid, bool& zero) {
-      const int m = mrow + 8 * h;                           // accumulator row == pixel / row inside the tile
-      zero = false;
-      if (a.conv == 1) {
-        const int srow = m_tile * a.box_r + m / 9;          // strip row
-        valid = m < a.box_r * 9 && srow < rows;
-        zero = (srow % 11) == 10;
-        grow = (long long)m_tile * a.box_r * 9 + m;
-      } else {
-        grow = (long long)m_tile * kTileM + m;
-        valid = grow < rows;
-      }
+    // accumulator row mrow + 8h: global output row (pixel / GEMM row), and whether it is inside the batch
+    auto out_row = [&](int h, long long& grow, bool& valid) {
+      grow = (long long)m_tile * kTileM + mrow + 8 * h;
+      valid = grow < rows;
     };
     // + skip stream, for both rows before the first output store.  The compiler keeps every load behind the stores that
     // precede it (a store might alias the skip stream), so loads interleaved with the stores would go out one round trip
@@ -272,8 +256,8 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         long long grow;
-        bool valid, zero;
-        out_row(h, grow, valid, zero);
+        bool valid;
+        out_row(h, grow, valid);
         if (!valid) continue;
         if (a.residual32) {
           const float* r32 = a.residual32 + grow * a.ldo;
@@ -295,8 +279,8 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       long long grow;                                       // global output row
-      bool valid, zero;
-      out_row(h, grow, valid, zero);
+      bool valid;
+      out_row(h, grow, valid);
       if (a.out_f32) {
         if (a.row_stats) {                                  // the 4 threads of a quad hold one row: reduce across them
           float mx = -INFINITY;
@@ -336,7 +320,6 @@ k_igemm(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtenso
           const int n = nb + 8 * j;
           float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
           if (a.relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
-          if (zero) { x0 = 0.f; x1 = 0.f; }
           *reinterpret_cast<__half2*>(o + n) = __floats2half2_rn(x0, x1);
           if (o32) *reinterpret_cast<float2*>(o32 + n) = make_float2(x0, x1);
         }

@@ -1,6 +1,6 @@
 // cz_nn.cu — policy + value network forward (agent/model.py:32-83) on H100 (sm_90a).
 //
-//   packed boards --k_conv_first--> strip activations (5x5 input conv over one-hot planes is a gather-sum
+//   packed boards --k_conv_first--> activations [B*90][C] (5x5 input conv over one-hot planes is a gather-sum
 //                                   of <= 25 weight rows per pixel; plane encoding never materialises)
 //   2 x blocks of  igemm::k_igemm   3x3 conv as implicit GEMM on wgmma (BN folded, +skip, ReLU fused)
 //   k_heads                         1x1 policy/value convs + BN + ReLU, value MLP + tanh
@@ -17,6 +17,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "cz_err.h"
@@ -85,25 +86,12 @@ int make_map_im2col(CUtensorMap* m, const void* base, int c, long long n_images,
   return 0;
 }
 
-// fp16 tensor [rows][w][c] (c contiguous), box {64, box_w, box_r}, 128B swizzle, zero OOB fill
-static int make_map_3d(CUtensorMap* m, const void* base, int c, int w, long long rows, int box_w, int box_r) {
-  if (load_encode()) return CZ_ERR_CUDA;
-  cuuint64_t dims[3] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)rows};
-  cuuint64_t strides[2] = {(cuuint64_t)c * 2, (cuuint64_t)c * 2 * w};
-  cuuint32_t box[3] = {64, (cuuint32_t)box_w, (cuuint32_t)box_r};
-  cuuint32_t es[3] = {1, 1, 1};
-  CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, es,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return cz_fail(CZ_ERR_CUDA, "cuTensorMapEncodeTiled(3d) failed: %d", (int)r);
-  return 0;
-}
-// fp16 matrix [rows][k] (k contiguous), box {64, box_rows}
-int make_map_2d(CUtensorMap* m, const void* base, int k, long long rows, int box_rows) {
+// fp16 matrix [rows][k] (k contiguous), box {64, rows_per_box}
+int make_map_2d(CUtensorMap* m, const void* base, int k, long long rows, int rows_per_box) {
   if (load_encode()) return CZ_ERR_CUDA;
   cuuint64_t dims[2] = {(cuuint64_t)k, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)k * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
+  cuuint32_t box[2] = {64, (cuuint32_t)rows_per_box};
   cuuint32_t es[2] = {1, 1};
   CUresult r = g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, es,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -171,11 +159,11 @@ static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const 
   CZ_CUDA(cudaGetLastError());
   return 0;
 }
-// With `out_map` (make_map_epi of a.out) the full M tiles of a dense conv that has fp16 output only and no skip stream leave
+// With `out_map` (make_map_epi of a.out) the full M tiles of a conv that has fp16 output only and no skip stream leave
 // through the staged epilogue.
 int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, const igemm::Args& a0, cudaStream_t st, const CUtensorMap* out_map) {
   igemm::Args a = a0;
-  a.staged = out_map && a.conv == 2 && !a.out_f32 && !a.residual && !a.residual32 && !a.out32;
+  a.staged = out_map && a.conv && !a.out_f32 && !a.residual && !a.residual32 && !a.out32;
   const CUtensorMap& tmOut = a.staged ? *out_map : tmA;    // not used unless staged
   switch (n_tile) {
     case 64: return launch_igemm_t<64>(tmA, tmB, tmOut, a, st);
@@ -194,37 +182,23 @@ static bool use_n_split(int n_boards, int c) {
   const int m_tiles = (n_boards * 90 + igemm::kTileM - 1) / igemm::kTileM;
   return m_tiles * (c / 64) <= num_sms();
 }
-// CZ_CONV_STRIP=1: the strip layout (separator row per board, tiled TMA) instead of the dense layout + im2col TMA
-static bool use_im2col() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("CZ_CONV_STRIP"); v = (e && e[0] == '1') ? 0 : 1; }
-  return v == 1;
-}
-
-static igemm::Args conv_args(int n_boards, int c, const float* bias, const __half* residual, __half* out, int relu) {
+igemm::Args conv_args(int n_boards, int c, const float* bias, const __half* residual, void* out, int relu) {
   igemm::Args a;
   memset(&a, 0, sizeof(a));
-  a.n_taps = 9; a.k_chunks = c / 64; a.box_w = 9; a.box_r = 14;
-  a.rows = n_boards * 11; a.m_tiles = (a.rows + 13) / 14; a.n_tiles = 1;
+  a.n_taps = 9; a.k_chunks = c / 64;
+  a.rows = n_boards * 90; a.m_tiles = (a.rows + 127) / 128; a.n_tiles = 1;
   a.n_total = c; a.n_valid = c; a.ldo = c; a.conv = 1; a.relu = relu; a.out_f32 = 0;
-  a.bias = bias; a.residual = residual; a.out = out; a.a_bytes = 64 * 9 * 14 * 2;
-  return a;
-}
-
-// dense pixel layout [n_boards*90][c] + im2col TMA
-static igemm::Args conv_args_dense(int n_boards, int c, const float* bias, const __half* residual, __half* out, int relu) {
-  igemm::Args a = conv_args(n_boards, c, bias, residual, out, relu);
-  a.conv = 2; a.rows = n_boards * 90; a.m_tiles = (a.rows + 127) / 128; a.a_bytes = 128 * 128;
+  a.bias = bias; a.residual = residual; a.out = out; a.rows_per_unit = 90;
   return a;
 }
 
 static igemm::Args dense_args(int m, int n_valid, int n_pad, int k_pad, int n_tile, const float* bias, float* out, int ldo) {
   igemm::Args a;
   memset(&a, 0, sizeof(a));
-  a.n_taps = 1; a.k_chunks = k_pad / 64; a.box_w = 1; a.box_r = 128;
+  a.n_taps = 1; a.k_chunks = k_pad / 64;
   a.rows = m; a.m_tiles = (m + 127) / 128; a.n_tiles = n_pad / n_tile;
   a.n_total = n_pad; a.n_valid = n_valid; a.ldo = ldo; a.conv = 0; a.relu = 0; a.out_f32 = 1;
-  a.bias = bias; a.residual = nullptr; a.out = out; a.a_bytes = 64 * 128 * 2;
+  a.bias = bias; a.residual = nullptr; a.out = out;
   return a;
 }
 
@@ -242,7 +216,7 @@ __device__ __forceinline__ int plane_of(uint8_t c) { return c == 0 ? -1 : ((c & 
 // select planes 14-27; board_stride = bytes between records.
 __global__ void k_conv_first(const uint8_t* __restrict__ boards, const __half* __restrict__ w,
                              const float* __restrict__ shift, __half* __restrict__ out, float* __restrict__ out32, int c_out,
-                             int board_pixels, int in_planes, int board_stride, const int* __restrict__ n_dev) {
+                             int in_planes, int board_stride, const int* __restrict__ n_dev) {
   if ((int)blockIdx.x >= __ldg(n_dev)) return;              // fixed-shape launch: the batch size lives on the device
   __shared__ int8_t pl[2][90];
   __shared__ uint16_t rows[90][52];
@@ -281,7 +255,7 @@ __global__ void k_conv_first(const uint8_t* __restrict__ boards, const __half* _
   const int c = 2 * (t % pairs), grp = t / pairs, n_groups = blockDim.x / pairs;
   if (grp >= n_groups) return;
   const float2 sh = *reinterpret_cast<const float2*>(shift + c);
-  __half* o = out + (size_t)b * board_pixels * c_out;
+  __half* o = out + (size_t)b * 90 * c_out;
   const __half2* w2 = reinterpret_cast<const __half2*>(w + c);
   const int stride2 = c_out / 2;
   for (int pix = p0 + grp; pix < p1; pix += n_groups) {
@@ -293,11 +267,8 @@ __global__ void k_conv_first(const uint8_t* __restrict__ boards, const __half* _
     }
     a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f);
     *reinterpret_cast<__half2*>(o + (size_t)pix * c_out + c) = __floats2half2_rn(a0, a1);
-    if (out32) *reinterpret_cast<float2*>(out32 + ((size_t)b * board_pixels + pix) * c_out + c) = make_float2(a0, a1);
+    if (out32) *reinterpret_cast<float2*>(out32 + ((size_t)b * 90 + pix) * c_out + c) = make_float2(a0, a1);
   }
-  if (blockIdx.y == 0)
-  for (int col = 90 + grp; col < board_pixels; col += n_groups)
-    *reinterpret_cast<__half2*>(o + (size_t)col * c_out + c) = __floats2half2_rn(0.f, 0.f);          // separator row (strip layout)
 }
 
 // one-hot planes [B][in_planes][10][9] f32 -> packed boards (inverse of state_to_planes / state_history_to_planes):
@@ -329,7 +300,7 @@ constexpr int kHeadPos = 4;
 constexpr int kMaxHeadOut = 36;                                   // 32 policy + 4 value channels
 static size_t heads_smem_bytes(int c_in, int n_out) { return ((size_t)kHeadPos * n_out * 90 + (size_t)(c_in / 8) * n_out * 8 + kHeadPos * 8) * sizeof(float); }
 __global__ void __launch_bounds__(256) k_heads(const __half* __restrict__ act, const float* __restrict__ act32, int c_in,
-                                                const int* __restrict__ n_dev, int board_pixels, int pol_c, int val_c, int pol_k1,
+                                                const int* __restrict__ n_dev, int pol_c, int val_c, int pol_k1,
                                                 const float* __restrict__ wh,      // [pol_c + val_c][c_in], BN scale folded
                                                 const float* __restrict__ shifth,  // [pol_c + val_c]
                                                 const float* __restrict__ wv1,     // [val_c * 90][H]
@@ -352,7 +323,7 @@ __global__ void __launch_bounds__(256) k_heads(const __half* __restrict__ act, c
   __syncthreads();
   for (int item = tid; item < npos * 90; item += 256) {
     const int p = item / 90, pix = item % 90;
-    const size_t row = ((size_t)(b0 + p) * board_pixels + pix) * c_in;
+    const size_t row = ((size_t)(b0 + p) * 90 + pix) * c_in;
     for (int o0 = 0; o0 < n_out; o0 += 6) {                  // six outputs per pass over the pixel's row (the row stays in L1)
       float s[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
 #pragma unroll 4
@@ -547,7 +518,7 @@ struct NnRuntime {
   uint64_t launches;
   // activations
   __half *x, *t, *y, *pol_feat;
-  float *x32, *y32;                      // fp32 skip stream (dense layout only)
+  float *x32, *y32;                      // fp32 skip stream
   float* logits;
   float2* stats;                         // [max_batch][kPolN / 256] softmax statistics of the policy GEMM's N tiles
   int* n_scalar;                         // device copy of a host-known batch size (reference-facing forward)
@@ -563,12 +534,11 @@ struct NnRuntime {
   __half* w_pol; float* b_pol;
   float* scratch;                            // 2*C floats for BN folding
   // tensor maps
-  CUtensorMap map_x, map_t, map_y, map_pf, map_wpol;
+  CUtensorMap map_pf, map_wpol;
   std::vector<CUtensorMap> map_w;
   std::vector<CUtensorMap> map_w_64;     // box rows = 64: 64-column tiles of the small-batch launches (use_n_split)
   bool fp32_skip;                        // keep the residual (skip) stream in fp32: halves the value error of deep nets, ~+30 % time
-  int board_pixels;                      // 99 = strip layout (separator row per board), 90 = dense + im2col TMA
-  CUtensorMap imap_x, imap_t, imap_y;    // im2col maps of the three activation buffers (dense layout)
+  CUtensorMap imap_x, imap_t, imap_y;    // im2col maps of the three activation buffers
   CUtensorMap emap_t;                    // conv1's output buffer as the staged conv epilogue stores it
   // optional CUDA-event timing of the residual-tower launches (bench.py roofline)
   bool profile;
@@ -608,12 +578,12 @@ static void prof_collect(NnRuntime* r) {
 
 static void layout(NnRuntime* r, Carver& cv) {
   const int c = r->filters;
-  const size_t act = (size_t)r->max_batch * 11 * 9 * c * sizeof(__half);
-  r->x = (__half*)cv.take(act);
-  r->t = (__half*)cv.take(act);
-  r->y = (__half*)cv.take(act);
-  r->x32 = (float*)cv.take(act * 2);
-  r->y32 = (float*)cv.take(act * 2);
+  const size_t act = (size_t)r->max_batch * 90 * c;       // elements of one activation buffer
+  r->x = (__half*)cv.take(act * sizeof(__half));
+  r->t = (__half*)cv.take(act * sizeof(__half));
+  r->y = (__half*)cv.take(act * sizeof(__half));
+  r->x32 = (float*)cv.take(act * sizeof(float));
+  r->y32 = (float*)cv.take(act * sizeof(float));
   r->pol_feat = (__half*)cv.take(((size_t)r->max_batch + 128) * 3 * r->pol_k1 * sizeof(__half));
   r->logits = (float*)cv.take((size_t)r->max_batch * kPolN * sizeof(float));
   r->stats = (float2*)cv.take((size_t)r->max_batch * (kPolN / 256) * sizeof(float2));
@@ -679,19 +649,12 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
   Carver cv{(uint8_t*)workspace, 0, bytes};
   layout(r, cv);
   const int c = filters;
-  const long long rows = (long long)max_batch * 11;
   int rc = 0;
-  r->board_pixels = use_im2col() ? 90 : 99;
-  if (r->board_pixels == 90) {
-    rc |= make_map_im2col(&r->imap_x, r->x, c, max_batch);
-    rc |= make_map_im2col(&r->imap_t, r->t, c, max_batch);
-    rc |= make_map_im2col(&r->imap_y, r->y, c, max_batch);
-    rc |= make_map_epi(&r->emap_t, r->t, c, (long long)max_batch * 90);
-  }
-  rc |= make_map_3d(&r->map_x, r->x, c, 9, rows, 9, 14);
-  rc |= make_map_3d(&r->map_t, r->t, c, 9, rows, 9, 14);
-  rc |= make_map_3d(&r->map_y, r->y, c, 9, rows, 9, 14);
-  rc |= make_map_3d(&r->map_pf, r->pol_feat, 3 * r->pol_k1, 1, (long long)max_batch + 128, 1, 128);
+  rc |= make_map_im2col(&r->imap_x, r->x, c, max_batch);
+  rc |= make_map_im2col(&r->imap_t, r->t, c, max_batch);
+  rc |= make_map_im2col(&r->imap_y, r->y, c, max_batch);
+  rc |= make_map_epi(&r->emap_t, r->t, c, (long long)max_batch * 90);
+  rc |= make_map_2d(&r->map_pf, r->pol_feat, 3 * r->pol_k1, (long long)max_batch + 128, 128);
   for (int net = n_nets - 1; net >= 0; --net) {
     select_net(r, net);
     rc |= make_map_2d(&r->map_wpol, r->w_pol, 3 * r->pol_k1, kPolN, 256);
@@ -704,10 +667,11 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
     store_net(r, net);
   }
   if (rc) { delete r; return nullptr; }
-  // separator rows and padding must start as zeros
-  cudaMemsetAsync(r->x, 0, (size_t)max_batch * 11 * 9 * c * 2, r->stream);
-  cudaMemsetAsync(r->t, 0, (size_t)max_batch * 11 * 9 * c * 2, r->stream);
-  cudaMemsetAsync(r->y, 0, (size_t)max_batch * 11 * 9 * c * 2, r->stream);
+  // the last, partial M tile of a conv or of the policy GEMM loads rows past the batch: they start as zeros, not as whatever
+  // the workspace held
+  cudaMemsetAsync(r->x, 0, (size_t)max_batch * 90 * c * 2, r->stream);
+  cudaMemsetAsync(r->t, 0, (size_t)max_batch * 90 * c * 2, r->stream);
+  cudaMemsetAsync(r->y, 0, (size_t)max_batch * 90 * c * 2, r->stream);
   cudaMemsetAsync(r->pol_feat, 0, ((size_t)max_batch + 128) * 3 * r->pol_k1 * 2, r->stream);
   return r;
 }
@@ -848,10 +812,10 @@ static int conv_first_threads(int c) {                    // (c/2) channel pairs
 }
 static int fw_first(NnRuntime* r, const uint8_t* boards, int n, const int* n_dev) {
   const int c = r->filters;
-  const bool s32 = r->board_pixels == 90 && r->fp32_skip;
+  const bool s32 = r->fp32_skip;
   int slices = (2 * num_sms() + n - 1) / n;                // >= 2 CTAs per SM in flight; big batches: one CTA per position
   if (slices > 15) slices = 15;
-  k_conv_first<<<dim3(n, slices), conv_first_threads(c), 0, r->stream>>>(boards, r->w_first, r->shift_first, r->x, s32 ? r->x32 : nullptr, c, r->board_pixels,
+  k_conv_first<<<dim3(n, slices), conv_first_threads(c), 0, r->stream>>>(boards, r->w_first, r->shift_first, r->x, s32 ? r->x32 : nullptr, c,
                                                             r->in_planes, (r->in_planes / 14) * CZ_BOARD_STRIDE, n_dev);
   r->launches++;
   CZ_CUDA(cudaGetLastError());
@@ -860,44 +824,29 @@ static int fw_first(NnRuntime* r, const uint8_t* boards, int n, const int* n_dev
 static int fw_tower(NnRuntime* r, int n, const int* n_dev) {
   const int c = r->filters;
   cudaStream_t st = r->stream;
-  const bool dense = r->board_pixels == 90;
-  const bool s32 = dense && r->fp32_skip;
-  float *x32 = s32 ? r->x32 : nullptr, *y32 = s32 ? r->y32 : nullptr;
+  float *x32 = r->fp32_skip ? r->x32 : nullptr, *y32 = r->fp32_skip ? r->y32 : nullptr;
   CUtensorMap *ix = &r->imap_x, *iy = &r->imap_y;
   __half *x = r->x, *y = r->y;
-  CUtensorMap *mx = &r->map_x, *my = &r->map_y;
+  const bool split = use_n_split(n, c);
+  const int nt = split ? 64 : c;
+  const std::vector<CUtensorMap>& wm = split ? r->map_w_64 : r->map_w;
   for (int i = 0; i < r->blocks; ++i) {
-    const size_t wsz = (size_t)c;
-    igemm::Args a1 = conv_args(n, c, r->shift_conv + (size_t)(2 * i) * wsz, nullptr, r->t, 1);
-    igemm::Args a2 = conv_args(n, c, r->shift_conv + (size_t)(2 * i + 1) * wsz, x, y, 1);
-    if (dense) {
-      igemm::Args d1 = conv_args_dense(n, c, a1.bias, nullptr, r->t, 1);
-      igemm::Args d2 = conv_args_dense(n, c, a2.bias, x, y, 1);
-      d1.n_dev = n_dev; d1.rows_per_unit = 90; d2.n_dev = n_dev; d2.rows_per_unit = 90;
-      d2.residual32 = x32; d2.out32 = y32;
-      { float* t32 = x32; x32 = y32; y32 = t32; }
-      // conv1: x -> t (no skip);  conv2: t (+ skip x or x32) -> y (+ y32)
-      const bool split = use_n_split(n, c);
-      const int nt = split ? 64 : c;
-      const std::vector<CUtensorMap>& wm = split ? r->map_w_64 : r->map_w;
-      d1.n_tiles = d2.n_tiles = c / nt;
-      if (launch_igemm(nt, *ix, wm[2 * i], d1, st, &r->emap_t)) return CZ_ERR_CUDA;
-      if (launch_igemm(nt, r->imap_t, wm[2 * i + 1], d2, st)) return CZ_ERR_CUDA;
-      CUtensorMap* ti = ix; ix = iy; iy = ti;
-    } else {
-      // strip layout (CZ_CONV_STRIP=1): host-known batch only
-      if (launch_igemm(c, *mx, r->map_w[2 * i], a1, st)) return CZ_ERR_CUDA;
-      if (launch_igemm(c, r->map_t, r->map_w[2 * i + 1], a2, st)) return CZ_ERR_CUDA;
-    }
+    // conv1: x -> t (no skip);  conv2: t (+ skip x or x32) -> y (+ y32)
+    igemm::Args d1 = conv_args(n, c, r->shift_conv + (size_t)(2 * i) * c, nullptr, r->t, 1);
+    igemm::Args d2 = conv_args(n, c, r->shift_conv + (size_t)(2 * i + 1) * c, x, y, 1);
+    d1.n_dev = d2.n_dev = n_dev;
+    d2.residual32 = x32; d2.out32 = y32;
+    d1.n_tiles = d2.n_tiles = c / nt;
+    if (launch_igemm(nt, *ix, wm[2 * i], d1, st, &r->emap_t)) return CZ_ERR_CUDA;
+    if (launch_igemm(nt, r->imap_t, wm[2 * i + 1], d2, st)) return CZ_ERR_CUDA;
     r->launches += 2;
-    __half* tx = x; x = y; y = tx;
-    CUtensorMap* tm = mx; mx = my; my = tm;
+    std::swap(x, y); std::swap(x32, y32); std::swap(ix, iy);
   }
   return 0;
 }
 static int fw_heads(NnRuntime* r, int n, const int* n_dev, float* value) {
   const int c = r->filters;
-  const bool s32 = r->board_pixels == 90 && r->fp32_skip;
+  const bool s32 = r->fp32_skip;
   const bool odd = (r->blocks & 1) != 0;                   // the tower ping-pongs x <-> y once per block
   const __half* x = odd ? r->y : r->x;
   const float* x32 = s32 ? (odd ? r->y32 : r->x32) : nullptr;
@@ -907,7 +856,7 @@ static int fw_heads(NnRuntime* r, int n, const int* n_dev, float* value) {
     r->heads_attr = true;
   }
   const int hp = n <= 2 * num_sms() ? 1 : kHeadPos;       // small batches: a block per position (same arithmetic per position)
-  k_heads<<<(n + hp - 1) / hp, 256, hsm, r->stream>>>(x, x32, c, n_dev, r->board_pixels, r->pol_c, r->val_c, r->pol_k1, r->wh, r->shifth,
+  k_heads<<<(n + hp - 1) / hp, 256, hsm, r->stream>>>(x, x32, c, n_dev, r->pol_c, r->val_c, r->pol_k1, r->wh, r->shifth,
                                                       r->wv1, r->bv1, r->wv2, r->bv2, r->value_fc, r->pol_feat, value, hp);
   igemm::Args ap = dense_args(n, kLabels, kPolN, 3 * r->pol_k1, 256, r->b_pol, r->logits, kPolN);
   ap.n_dev = n_dev; ap.rows_per_unit = 1; ap.row_stats = r->stats;
@@ -945,9 +894,6 @@ static int forward_tower(NnRuntime* r, const uint8_t* boards, int n_max, const i
 // host-known batch: the reference-facing predict_on_batch (api.py:62-64) -> the full softmax vector
 static int forward_chunk(NnRuntime* r, const uint8_t* boards, int n, float* policy, float* value) {
   k_set_int<<<1, 1, 0, r->stream>>>(r->n_scalar, n);
-  if (r->board_pixels != 90) {                      // strip-layout baselines launch exact shapes
-    // (the device-side batch size is still honoured by the first conv, the heads and the policy GEMM)
-  }
   const int rc = forward_tower(r, boards, n, r->n_scalar, value);
   if (rc) return rc;
   k_softmax<<<n, 256, 0, r->stream>>>(r->logits, kPolN, r->stats, kPolN / 256, policy);
@@ -988,7 +934,6 @@ int nn_forward_leaves(NnRuntime* r, int net, int part, const uint8_t* boards, in
                       const int32_t* label_counts, float* legal_p, float* value) {
   if (!r || net < 0 || net >= r->n_nets) return cz_fail(CZ_ERR_STATE, "no such network");
   if (n_max > r->max_batch) return cz_fail(CZ_ERR_ARG, "nn_forward_leaves: %d leaves > max batch %d", n_max, r->max_batch);
-  if (r->board_pixels != 90) return cz_fail(CZ_ERR_UNSUPPORTED, "nn_forward_leaves needs the dense (im2col) layout");
   select_net(r, net);
   if (!r->ready) return cz_fail(CZ_ERR_STATE, "network weights not set (cz_nn_set_weights)");
   int rc = 0;
@@ -1003,13 +948,11 @@ int nn_forward_leaves(NnRuntime* r, int net, int part, const uint8_t* boards, in
 }
 void nn_set_capturing(NnRuntime* r, bool on) { if (r) r->capturing = on; }
 bool nn_profiling(const NnRuntime* r) { return r && r->profile; }
-void nn_set_stream(NnRuntime* r, void* stream) { if (r) r->stream = (cudaStream_t)stream; }
 // Parity tests: copy rows of an intermediate buffer out after a forward.  Which physical buffer holds a stage follows the
 // ping-pong of fw_tower and the choice fw_heads makes (x <-> y once per block, the fp32 copies alongside).  Off the forward
 // path: nothing here runs unless a test asks.
 int nn_read_buffer(NnRuntime* r, int which, int n, void* dst, long long dst_bytes, long long* row_bytes) {
   if (!r) return cz_fail(CZ_ERR_STATE, "cz_nn_read_buffer: engine has no network");
-  if (r->board_pixels != 90) return cz_fail(CZ_ERR_UNSUPPORTED, "cz_nn_read_buffer: strip layout (CZ_CONV_STRIP=1)");
   const bool s32 = r->fp32_skip, odd = (r->blocks & 1) != 0;
   const long long act = 90LL * r->filters;
   const void* src = nullptr;
@@ -1055,21 +998,9 @@ double nn_tower_flops_per_position(const NnRuntime* r) { return r ? 2.0 * 90.0 *
 // Building blocks exported for parity tests and profiling (not part of the reference-facing surface).
 extern "C" {
 
-// 3x3 "same" convolution on strip-layout activations: out = relu?(conv(in, w) + bias (+ residual)).
-//   act_in/out/residual: fp16 [n_boards*11][9][c] (separator rows of act_in must be zero)
-//   w: fp16 [9][c_out = c][c_in = c] ; bias f32 [c]
-int cz_igemm_conv3x3(const void* act_in, const void* w, const float* bias, const void* residual, void* act_out,
-                     int n_boards, int c, int relu, void* stream) {
-  using namespace cznn;
-  if (c % 64 || c < 64 || c > 256 || n_boards <= 0) return cz_fail(CZ_ERR_ARG, "cz_igemm_conv3x3: bad shape");
-  CUtensorMap ma, mb;
-  if (make_map_3d(&ma, act_in, c, 9, (long long)n_boards * 11, 9, 14)) return CZ_ERR_CUDA;
-  igemm::Args a = conv_args(n_boards, c, bias, (const __half*)residual, (__half*)act_out, relu);
-  if (make_map_2d(&mb, w, c, 9LL * c, c)) return CZ_ERR_CUDA;
-  return launch_igemm(c, ma, mb, a, (cudaStream_t)stream);
-}
-
-// Same convolution on DENSE activations fp16 [n_boards][10][9][c] through the im2col TMA path.
+// 3x3 "same" convolution on activations fp16 [n_boards][10][9][c] through the im2col TMA path:
+// out = relu?(conv(in, w) + bias (+ residual)); residual and out have the layout of in; w: fp16 [9][c_out = c][c_in = c],
+// bias f32 [c].
 int cz_igemm_conv3x3_dense(const void* act_in, const void* w, const float* bias, const void* residual, void* act_out,
                            int n_boards, int c, int relu, void* stream) {
   using namespace cznn;
@@ -1077,7 +1008,7 @@ int cz_igemm_conv3x3_dense(const void* act_in, const void* w, const float* bias,
   CUtensorMap ma, mb;
   if (make_map_im2col(&ma, act_in, c, n_boards)) return CZ_ERR_CUDA;
   if (make_map_2d(&mb, w, c, 9LL * c, c)) return CZ_ERR_CUDA;
-  igemm::Args a = conv_args_dense(n_boards, c, bias, (const __half*)residual, (__half*)act_out, relu);
+  igemm::Args a = conv_args(n_boards, c, bias, (const __half*)residual, act_out, relu);
   return launch_igemm(c, ma, mb, a, (cudaStream_t)stream);
 }
 
@@ -1088,7 +1019,7 @@ int cz_igemm_dense(const void* a_dev, const void* w_dev, const float* bias, floa
   using namespace cznn;
   if (k % 64 || n_pad % n_tile || m <= 0) return cz_fail(CZ_ERR_ARG, "cz_igemm_dense: bad shape");
   CUtensorMap ma, mb;
-  if (make_map_3d(&ma, a_dev, k, 1, (long long)m, 1, 128)) return CZ_ERR_CUDA;
+  if (make_map_2d(&ma, a_dev, k, (long long)m, 128)) return CZ_ERR_CUDA;
   if (make_map_2d(&mb, w_dev, k, n_pad, n_tile)) return CZ_ERR_CUDA;
   igemm::Args a = dense_args(m, n_valid, n_pad, k, n_tile, bias, out, ldo);
   return launch_igemm(n_tile, ma, mb, a, (cudaStream_t)stream);

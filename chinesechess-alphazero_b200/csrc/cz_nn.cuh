@@ -34,7 +34,6 @@ void nn_prof_begin(NnRuntime*, double flops);   // event bracket around the towe
 void nn_prof_end(NnRuntime*);
 int nn_launches_per_forward(const NnRuntime*);
 double nn_tower_flops_per_position(const NnRuntime*);
-void nn_set_stream(NnRuntime*, void* stream);
 uint64_t nn_launches(const NnRuntime*);
 void nn_profile(NnRuntime*, bool on);
 int nn_profile_read(NnRuntime*, double* ms, uint64_t* launches, double* flops);

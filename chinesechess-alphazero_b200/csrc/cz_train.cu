@@ -692,12 +692,8 @@ static int bn_backward(Trainer* t, Bn& b, long long P, const float* skip, const 
 }
 
 static igemm::Args conv_args(int n, int c, float* out) {
-  igemm::Args a;
-  memset(&a, 0, sizeof(a));
-  a.n_taps = 9; a.k_chunks = c / 64; a.box_w = 9; a.box_r = 14;
-  a.rows = n * 90; a.m_tiles = (a.rows + 127) / 128; a.n_tiles = 1;
-  a.n_total = c; a.n_valid = c; a.ldo = c; a.conv = 2; a.relu = 0; a.out_f32 = 1;
-  a.out = out; a.a_bytes = 128 * 128; a.rows_per_unit = 90;
+  igemm::Args a = cznn::conv_args(n, c, nullptr, nullptr, out, 0);
+  a.out_f32 = 1;
   return a;
 }
 

@@ -38,8 +38,8 @@ CZ_KERNEL(k_pv)(EngineDev E, int g, int max_len, cz_pv_info* out) {
   const int len = game_pv(E, g, max_len, out->moves, &v, &has, tree_smem());
   if (czs::lane() == 0) { out->n_moves = len; out->value = v; out->has_value = has; }
 }
-// The search kernels work on a game range [g0, g1) ("slot"): cz_search pipelines two halves of the games so the tree
-// work of one half overlaps the network evaluation of the other.  Per-game results do not depend on the split.
+// The search kernels work on a game range [g0, g1): in arena mode the device-driven loop evaluates each half of the games
+// with its own network.  Per-game results do not depend on the split.
 CZ_KERNEL(k_wave)(EngineDev E, int g0, int g1) {
   const int g = g0 + my_game();
   if (g >= g1) return;
@@ -83,8 +83,8 @@ CZ_KERNEL(k_scan)(EngineDev E, int gb, int ge, int slot) {
 #endif
   }
 }
-// dense leaf list of a range: boards, and (labels != null) the action labels of each leaf's legal moves in edge order, which
-// is all the evaluation step has to know to hand back exactly the priors the search will read
+// dense leaf list of a range: boards, and the action labels of each leaf's legal moves in edge order, which is all the
+// evaluation step has to know to hand back exactly the priors the search will read
 #if !defined(CZ_EMUL)
 // The same scan with one thread per game (1024 threads, chunked): the single-warp version walks 32 dependent chunks at
 // 1024 games (52 us in the c3 launch list); this one is a couple of microseconds.  Same outputs, same counters.
@@ -125,17 +125,15 @@ CZ_KERNEL(k_gather)(EngineDev E, int g0, int g1, uint8_t* dense, int16_t* labels
     const uint8_t* s = E.leaf_board + ((size_t)g * E.K + j) * E.lb_stride;
     uint8_t* d = dense + (size_t)(off + j) * E.lb_stride;
     if (czs::lane() < E.lb_stride / 16) reinterpret_cast<uint4*>(d)[czs::lane()] = reinterpret_cast<const uint4*>(s)[czs::lane()];
-    if (labels) {
-      const int node = E.sim_leaf_node[(size_t)g * E.K + E.leaf_sim[(size_t)g * E.K + j]];
-      const size_t ni = (size_t)g * E.ncap + node;
-      const int L = (int)(E.node_meta[ni] & 0xff);
-      const size_t eo = (size_t)g * E.ecap + E.node_edge_off[ni];
-      for (int i = czs::lane(); i < L; i += 32) {
-        const move_t m = E.edge_move[eo + i];
-        labels[(size_t)(off + j) * MAX_MOVES + i] = E.label_lut[mv_from(m) * 90 + mv_to(m)];
-      }
-      if (czs::lane() == 0) nlab[off + j] = L;
+    const int node = E.sim_leaf_node[(size_t)g * E.K + E.leaf_sim[(size_t)g * E.K + j]];
+    const size_t ni = (size_t)g * E.ncap + node;
+    const int L = (int)(E.node_meta[ni] & 0xff);
+    const size_t eo = (size_t)g * E.ecap + E.node_edge_off[ni];
+    for (int i = czs::lane(); i < L; i += 32) {
+      const move_t m = E.edge_move[eo + i];
+      labels[(size_t)(off + j) * MAX_MOVES + i] = E.label_lut[mv_from(m) * 90 + mv_to(m)];
     }
+    if (czs::lane() == 0) nlab[off + j] = L;
   }
 }
 // Device-driven search loop: after every iteration tell the polling host thread (mapped pinned memory) how many iterations
@@ -331,7 +329,7 @@ struct cz_engine {
   cz_pv_info* pv_dev;
   unsigned long long* stat_out;
   cz_root_info* root_info_dev;
-  float* policy_buf; float* value_buf;                      // evaluator outputs for the built-in network
+  float* value_buf;                                         // [G*K] values of the built-in network (integrated search)
   float* legal_p;                                           // [G*K][MAX_MOVES] priors of the legal moves (integrated search)
   uint8_t* board_stage;                                     // [G][96] staging for reset / set_root
   int32_t* stat_n; uint16_t* stat_mv; int32_t* stat_cnt;    // staging for cz_get_root_stats
@@ -345,18 +343,14 @@ struct cz_engine {
 #if !defined(CZ_EMUL)
   cznn::NnRuntime* nn;
   size_t nn_bytes;
-  cudaStream_t tree_stream;                                 // second stream for the pipelined search (NULL = off)
-  cudaEvent_t ev_ready[2], ev_done[2];
-  int32_t* h_totals;                                        // pinned [8]
   // device-driven search loop: one iteration = three captured graphs per game range (tree work + first conv | residual
   // tower | heads + legal priors), launched back to back; the host only polls h_flags (mapped pinned memory)
   cudaGraphExec_t g_pre[2], g_tower[2], g_post[2];
   cudaGraphExec_t g_while;                                  // the whole loop as one graph: WHILE conditional node around the iteration
   unsigned long long while_handle;
   int capture_cond;                                         // 1 while capturing the body of g_while (k_loop_flag sets the condition)
-  int loop_mode;                                            // 0 host-driven (round 1), 1 sub-graphs + flag polling, 2 WHILE graph
   int n_ranges;                                             // 1, or 2 in arena mode (one network per range)
-  bool graphs_built, graph_loop;
+  bool graphs_built;
   volatile int32_t* h_flags;                                // mapped pinned [4]: iterations finished, busy
   int32_t* d_flags;                                         // device view of h_flags
 #endif
@@ -413,11 +407,10 @@ size_t carve(cz_engine* e, uint8_t* base) {
   e->sims_stage = cv.take<int32_t>(G);
   e->stat_n = cv.take<int32_t>(G * MAX_MOVES); e->stat_mv = cv.take<uint16_t>(G * MAX_MOVES); e->stat_cnt = cv.take<int32_t>(G);
   if (c.nn_filters > 0) {
-    e->policy_buf = cv.take<float>(G * K * (size_t)CZ_N_LABELS);
     e->value_buf = cv.take<float>(G * K);
     e->legal_p = cv.take<float>(G * K * (size_t)MAX_MOVES);
   } else {
-    e->policy_buf = nullptr; e->value_buf = nullptr; e->legal_p = nullptr;
+    e->value_buf = nullptr; e->legal_p = nullptr;
   }
   visits_carve(d.sp, cv, c);
   return cv.off + 1024;
@@ -510,12 +503,9 @@ int cz_create(const cz_config* cfg, void* workspace, uint64_t workspace_bytes, v
   d.seed = cfg->seed; d.rank = cfg->rank; d.arena = cfg->arena ? 1 : 0;
   const size_t used = carve(e, e->ws);
 #if !defined(CZ_EMUL)
-  e->nn = nullptr; e->nn_bytes = 0; e->tree_stream = nullptr; e->h_totals = nullptr;
+  e->nn = nullptr; e->nn_bytes = 0;
   e->graphs_built = false; e->h_flags = nullptr; e->d_flags = nullptr; e->n_ranges = cfg->arena ? 2 : 1;
   for (int i = 0; i < 2; ++i) { e->g_pre[i] = e->g_tower[i] = e->g_post[i] = nullptr; }
-  // CZ_SEARCH_LOOP = while (default: one graph launch per search, loop on the device) | graph (three sub-graphs per iteration,
-  // the host polls a mapped flag; also what runs while cz_nn_profile brackets the tower) | host (round-1 host-driven loops)
-  { const char* m = getenv("CZ_SEARCH_LOOP"); e->loop_mode = (m && m[0] == 'h') ? 0 : (m && m[0] == 'g') ? 1 : 2; e->graph_loop = e->loop_mode != 0; }
   e->g_while = nullptr; e->while_handle = 0; e->capture_cond = 0;
   if (cudaSetDevice(cfg->device) != cudaSuccess) { delete e; return cz_fail(CZ_ERR_CUDA, "cz_create: cudaSetDevice(%d) failed", cfg->device); }
   if (!e->stream) {
@@ -526,15 +516,6 @@ int cz_create(const cz_config* cfg, void* workspace, uint64_t workspace_bytes, v
     e->own_stream = true;
   }
   if (cfg->nn_filters > 0) {
-    const char* off = getenv("CZ_NO_PIPELINE");
-    if (!(off && off[0] == '1')) {
-      if (cudaStreamCreateWithFlags(&e->tree_stream, cudaStreamNonBlocking) != cudaSuccess) e->tree_stream = nullptr;
-      for (int i = 0; i < 2; ++i) {
-        cudaEventCreateWithFlags(&e->ev_ready[i], cudaEventDisableTiming);
-        cudaEventCreateWithFlags(&e->ev_done[i], cudaEventDisableTiming);
-      }
-    }
-    if (cudaMallocHost((void**)&e->h_totals, 8 * sizeof(int32_t)) != cudaSuccess) { delete e; return cz_fail(CZ_ERR_CUDA, "cz_create: cudaMallocHost failed"); }
     void* hf = nullptr;
     if (cudaHostAlloc(&hf, 64, cudaHostAllocMapped) != cudaSuccess || cudaHostGetDevicePointer((void**)&e->d_flags, hf, 0) != cudaSuccess) {
       delete e; return cz_fail(CZ_ERR_CUDA, "cz_create: mapped host memory for the loop flags failed");
@@ -574,12 +555,6 @@ void cz_destroy(cz_engine* e) {
   if (!e) return;
 #if !defined(CZ_EMUL)
   cznn::nn_destroy(e->nn);
-  if (e->tree_stream) {
-    cudaStreamSynchronize(e->tree_stream);
-    cudaStreamDestroy(e->tree_stream);
-    for (int i = 0; i < 2; ++i) { cudaEventDestroy(e->ev_ready[i]); cudaEventDestroy(e->ev_done[i]); }
-  }
-  if (e->h_totals) cudaFreeHost(e->h_totals);
   if (e->h_flags) cudaFreeHost((void*)e->h_flags);
   if (e->own_stream) { cudaStreamSynchronize(e->stream); cudaStreamDestroy(e->stream); }
   for (int i = 0; i < 2; ++i) {
@@ -749,63 +724,6 @@ int cz_search_apply_legal(cz_engine* e, const float* legal_p_dev, const float* v
 
 #if !defined(CZ_EMUL)
 namespace {
-// Two halves of the games ("slots") alternate between tree work (stream T) and network evaluation (the engine stream):
-//   T: wave/scan/gather(h)  -> host reads the leaf count -> N: forward(h) -> T: apply(h), wave(h) ...
-// while N evaluates one half the other half walks its trees, so the tensor cores never wait for the integer kernels.
-int search_pipelined(cz_engine* e) {
-  const int G = e->cfg.n_games, K = e->cfg.leaves_per_round;
-  const int mid = (G + 1) / 2;
-  const int gb[2] = {0, mid}, ge[2] = {mid, G};
-  uint8_t* dense[2] = {e->d.leaf_dense, e->d.leaf_dense + (size_t)mid * K * e->d.lb_stride};
-  float* pol[2] = {e->policy_buf, e->policy_buf + (size_t)mid * K * CZ_N_LABELS};
-  float* val[2] = {e->value_buf, e->value_buf + (size_t)mid * K};
-  cudaStream_t T = e->tree_stream, N = e->stream;
-  cudaEvent_t ready[2] = {e->ev_ready[0], e->ev_ready[1]};   // gather(h) done on T
-  cudaEvent_t done[2] = {e->ev_done[0], e->ev_done[1]};      // forward(h) done on N
-  int n_in_flight[2] = {0, 0};
-  bool busy[2] = {true, true};
-  // everything queued on the engine stream so far (begin kernels) must precede the tree stream's first wave
-  cudaEventRecord(e->ev_done[0], N);
-  cudaStreamWaitEvent(T, e->ev_done[0], 0);
-  for (int turn = 0;; ++turn) {
-    const int h = turn & 1;
-    if (!busy[0] && !busy[1] && n_in_flight[0] == 0 && n_in_flight[1] == 0) break;
-    if (!busy[h] && n_in_flight[h] == 0) continue;
-    if (n_in_flight[h] > 0) {                                 // evaluation of this half is (being) computed on N
-      cudaStreamWaitEvent(T, done[h], 0);
-      RANGE_LAUNCH(e, T, gb[h], ge[h], k_apply, e->d, gb[h], ge[h], (const float*)pol[h], (const float*)nullptr, (const float*)val[h]);
-      e->launches += 1;
-      n_in_flight[h] = 0;
-    }
-    RANGE_LAUNCH(e, T, gb[h], ge[h], k_wave, e->d, gb[h], ge[h]);
-    CZ_LAUNCH(k_scan, 1, 1, 0, T, e->d, gb[h], ge[h], h);
-    RANGE_LAUNCH(e, T, gb[h], ge[h], k_gather, e->d, gb[h], ge[h], dense[h], (int16_t*)nullptr, (int32_t*)nullptr);
-    cudaMemcpyAsync(e->h_totals + 4 * h, e->d.totals + 4 * h, 2 * sizeof(int32_t), cudaMemcpyDeviceToHost, T);
-    cudaEventRecord(ready[h], T);
-    e->launches += 3;
-    if (cudaStreamSynchronize(T) != cudaSuccess) return cz_fail(CZ_ERR_CUDA, "cz_search: device failure in the tree stream");
-    const int n = e->h_totals[4 * h];
-    busy[h] = e->h_totals[4 * h + 1] != 0 || n > 0;
-    if (n > 0) {
-      cudaStreamWaitEvent(N, ready[h], 0);
-      const int rc = cznn::nn_forward_boards(e->nn, e->cfg.arena ? h : 0, dense[h], n, pol[h], val[h]);   // arena: range h = player h's trees
-      if (rc) return rc;
-      cudaEventRecord(done[h], N);
-      n_in_flight[h] = n;
-    }
-  }
-  // leave both streams quiescent and ordered for the caller
-  cudaEventRecord(ready[0], T);
-  cudaStreamWaitEvent(N, ready[0], 0);
-  const char* msg;
-  if (czrt_last_error(&msg)) return cz_fail(CZ_ERR_CUDA, "cz_search: %s", msg);
-  return 0;
-}
-}  // namespace
-#endif
-
-#if !defined(CZ_EMUL)
-namespace {
 // ---- device-driven search loop ------------------------------------------------------------------------------------------
 // Range h = games [gb, ge) evaluated by network h (arena: player h's trees; otherwise one range = all games).  One iteration
 // of a range:   apply(previous evaluation) -> wave -> scan -> gather(+labels) -> first conv | tower | heads, policy GEMM,
@@ -946,7 +864,7 @@ int search_graph_loop(cz_engine* e) {
     }
     if (!e->graphs_built) {
       int rc = build_graphs(e);
-      if (!rc && e->loop_mode == 2) rc = build_while_graph(e);
+      if (!rc) rc = build_while_graph(e);
       if (rc) return rc;
     }
     ++launched;
@@ -982,25 +900,7 @@ int cz_search(cz_engine* e, const cz_root_opts* opts) {
   if (!e->nn || !cznn::nn_ready(e->nn)) return cz_fail(CZ_ERR_STATE, "cz_search: network weights not set");
   int rc = cz_search_begin(e, opts);
   if (rc) return rc;
-  if (e->graph_loop) return search_graph_loop(e);
-  // ---- round-1 host-driven loops (CZ_SEARCH_LOOP=host), kept as the A/B baseline: the full softmax vector per leaf, one
-  // stream synchronisation per wave
-  // two half-ranges only pay when each half still fills the tensor cores (>= 4096 leaves per round); the arena always
-  // needs them (one range per network)
-  const char* force = getenv("CZ_FORCE_PIPELINE");                 // test hook: the two-range path at any size
-  if (e->tree_stream && ((long long)e->cfg.n_games * e->cfg.leaves_per_round >= 8192 || e->cfg.arena || (force && force[0] == '1')))
-    return search_pipelined(e);
-  if (e->cfg.arena) return cz_fail(CZ_ERR_STATE, "cz_search: arena mode needs the two-range pipeline (CZ_NO_PIPELINE is set)");
-  for (;;) {
-    int32_t n = 0, busy = 0;
-    if ((rc = cz_search_wave(e, &n, &busy))) return rc;
-    if (n > 0) {
-      if ((rc = cznn::nn_forward_boards(e->nn, 0, e->d.leaf_dense, n, e->policy_buf, e->value_buf))) return rc;
-      if ((rc = cz_search_apply(e, e->policy_buf, e->value_buf))) return rc;
-    }
-    if (!busy) break;
-  }
-  return 0;
+  return search_graph_loop(e);
 #endif
 }
 
@@ -1012,19 +912,7 @@ int cz_search_run(cz_engine* e) {
   if (!e) return cz_fail(CZ_ERR_ARG, "cz_search_run: null engine");
   if (!e->nn || !cznn::nn_ready(e->nn)) return cz_fail(CZ_ERR_STATE, "cz_search_run: network weights not set");
   if (e->last_leaves != 0) return cz_fail(CZ_ERR_STATE, "cz_search_run: %d leaves of a host-driven wave were not applied", e->last_leaves);
-  if (e->graph_loop) return search_graph_loop(e);
-  if (e->cfg.arena) return cz_fail(CZ_ERR_UNSUPPORTED, "cz_search_run: the host-driven loop (CZ_SEARCH_LOOP=host) serves arena engines through cz_search only");
-  for (;;) {
-    int32_t n = 0, busy = 0;
-    int rc;
-    if ((rc = cz_search_wave(e, &n, &busy))) return rc;
-    if (n > 0) {
-      if ((rc = cznn::nn_forward_boards(e->nn, 0, e->d.leaf_dense, n, e->policy_buf, e->value_buf))) return rc;
-      if ((rc = cz_search_apply(e, e->policy_buf, e->value_buf))) return rc;
-    }
-    if (!busy) break;
-  }
-  return 0;
+  return search_graph_loop(e);
 #endif
 }
 

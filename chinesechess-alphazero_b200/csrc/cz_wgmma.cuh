@@ -56,12 +56,6 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* t, uin
       ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(t)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* t, uint64_t* bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(t)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 // Tensor store shared -> global of one box at {c0, c1}.  Stores are tracked in the issuing thread's bulk groups: commit, then
 // wait_group_read<N> until all but the N latest groups have finished READING shared memory (the source may be rewritten; the
 // data need not have landed), or wait_group_all until every group is complete (before the thread exits).

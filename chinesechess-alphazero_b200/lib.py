@@ -136,7 +136,6 @@ _SIGS = {
     "cz_launch_count": (C.c_int, [_P, C.POINTER(C.c_uint64)]),
     "cz_nn_profile": (C.c_int, [_P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.POINTER(C.c_double)]),
     "cz_noise_sample": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P]),
-    "cz_igemm_conv3x3": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "cz_igemm_conv3x3_dense": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P]),
     "cz_igemm_dense": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P]),
     "cz_nn_read_buffer": (C.c_int, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
@@ -155,7 +154,7 @@ _SIGS = {
     "cz_train_bn": (C.c_int, [_P, C.c_longlong, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
 }
 # entry points that only exist in the CUDA build (tensor cores cannot be emulated on the CPU)
-CUDA_ONLY = {"cz_igemm_conv3x3", "cz_igemm_conv3x3_dense", "cz_igemm_dense", "cz_train_workspace_bytes", "cz_train_create",
+CUDA_ONLY = {"cz_igemm_conv3x3_dense", "cz_igemm_dense", "cz_train_workspace_bytes", "cz_train_create",
              "cz_train_destroy", "cz_train_set_params", "cz_train_step", "cz_train_read_grad", "cz_train_read_buffer", "cz_train_wgrad3x3",
              "cz_train_dgrad3x3", "cz_train_bn", "cz_train_set_adam", "cz_train_adam_iterations"}
 

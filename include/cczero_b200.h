@@ -233,9 +233,11 @@ int cz_search_more(cz_engine* e, int32_t n_sims);
  * per-game read position is kept.  Stream-ordered. */
 int cz_set_noise_table(cz_engine* e, const double* noise_dev, int64_t noise_stride);
 /* Whole search with the built-in network as evaluator (needs cz_nn_set_weights).  Device-driven: every wave / evaluation /
- * apply iteration is a fixed-shape sequence of launches (captured CUDA graphs) whose batch size is a device integer; the host
- * thread only polls a flag in mapped memory to learn that no game has work left.  Synchronises once, at the end.
- * (CZ_SEARCH_LOOP=host in the environment at cz_create selects the round-1 host-driven loop: the A/B baseline.) */
+ * apply iteration is a fixed-shape sequence of launches whose batch size is a device integer, captured as CUDA graphs.  A
+ * search is one launch of a graph whose WHILE node repeats the iteration until no game has work left.  The engine's first
+ * search runs one iteration as plain launches, captures the graphs, and runs the rest as three sub-graphs per iteration while
+ * the host polls a flag in mapped memory; so does every search while cz_nn_profile is on (events bracket the tower).
+ * Synchronises once, at the end. */
 int cz_search(cz_engine* e, const cz_root_opts* opts);
 /* The loop of cz_search alone: run the simulations cz_search_begin / cz_search_more queued, built-in network as evaluator.
  * (A UCI front end slices action()'s rounds with cz_search_more and prints `info depth` lines in between.)  Synchronises. */
@@ -369,12 +371,8 @@ int cz_launch_count(cz_engine* e, uint64_t* n);
  * Tensor-core building blocks, exported for parity tests and profiling of the dominant kernel
  * (the residual-block convolutions of agent/model.py:68-83 and the policy Dense of :54).
  * ---------------------------------------------------------------------------------------- */
-/* 3x3 "same" convolution + bias (+ residual) (+ ReLU) on fp16 strip-layout activations
- * [n_boards*11][9][c] (row b*11+10 of every board is an all-zero separator); w fp16 [9][c][c]
- * = [tap kh*3+kw][c_out][c_in]; bias f32 [c]. */
-int cz_igemm_conv3x3(const void* act_in_dev, const void* w_dev, const float* bias_dev, const void* residual_dev,
-                     void* act_out_dev, int n_boards, int c, int relu, void* stream);
-/* Same convolution on dense activations fp16 [n_boards][10][9][c] (no separator rows), fed by im2col-mode TMA. */
+/* 3x3 "same" convolution + bias (+ residual) (+ ReLU) on fp16 activations [n_boards][10][9][c], fed by im2col-mode TMA;
+ * w fp16 [9][c][c] = [tap kh*3+kw][c_out][c_in]; bias f32 [c]. */
 int cz_igemm_conv3x3_dense(const void* act_in_dev, const void* w_dev, const float* bias_dev, const void* residual_dev,
                            void* act_out_dev, int n_boards, int c, int relu, void* stream);
 /* `count` draws of the on-device root-noise sampler (noise_mode 1): the first component of
@@ -407,7 +405,7 @@ typedef enum cz_nn_buffer {
 } cz_nn_buffer;
 /* Copy the first n position rows of buffer `which` (cz_nn_buffer) to dst_dev; *row_bytes = bytes per row.  dst_dev = NULL
  * only reports row_bytes.  CZ_ERR_ARG: unknown buffer, n > max batch or dst_bytes < n * row_bytes; CZ_ERR_STATE: the
- * buffer does not exist in this configuration; CZ_ERR_UNSUPPORTED: strip layout (CZ_CONV_STRIP=1).  Synchronises. */
+ * buffer does not exist in this configuration.  Synchronises. */
 int cz_nn_read_buffer(cz_engine* e, int32_t which, int32_t n, void* dst_dev, int64_t dst_bytes, int64_t* row_bytes);
 
 /* ------------------------------------------------------------------------------------------

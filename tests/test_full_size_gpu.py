@@ -37,8 +37,8 @@ def _roots(eng):
 
 def test_c3_full_size_replicas_agree_and_match_a_single_game(cuda_lib):
     """Root noise off: all 1024 games are the SAME search.  (a) every game's root statistics are bit-identical, (b) and
-    identical to ONE game searched alone in its own engine — batch composition (8192 leaves per round vs 8), the
-    two-range pipeline and the tile a position lands in must not leak into a game, (c) visits are conserved."""
+    identical to ONE game searched alone in its own engine — batch composition (8192 leaves per round vs 8) and the tile
+    a position lands in must not leak into a game, (c) visits are conserved."""
     w = _weights()
     eng = _engine(cuda_lib, G, w, noise_eps=0.0)
     eng.search(None)

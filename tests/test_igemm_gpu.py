@@ -53,39 +53,6 @@ def _conv_ref_and_scale(x, w, bias, res, relu):
     return (ref.relu() if relu else ref), scale
 
 
-def _strip_from_nchw(x):
-    """[B,C,10,9] f32 -> fp16 strip [B*11,9,C] with zero separator rows."""
-    b, c = x.shape[0], x.shape[1]
-    s = torch.zeros(b, 11, 9, c, device=x.device, dtype=torch.half)
-    s[:, :10] = x.permute(0, 2, 3, 1).half()
-    return s.reshape(b * 11, 9, c).contiguous()
-
-
-def _nchw_from_strip(s, b, c):
-    return s.reshape(b, 11, 9, c)[:, :10].permute(0, 3, 1, 2).float()
-
-
-@pytest.mark.parametrize("n_boards,c,residual,relu", [(1, 128, False, True), (5, 256, True, True), (29, 128, True, False),
-                                                       (64, 256, False, False), (200, 192, True, True), (3, 64, True, True)])
-def test_conv3x3_matches_torch(cuda_lib, n_boards, c, residual, relu):
-    g = torch.Generator(device="cuda").manual_seed(n_boards * 1000 + c)
-    x = torch.randn(n_boards, c, 10, 9, device="cuda", generator=g).half().float()
-    w = (torch.randn(c, c, 3, 3, device="cuda", generator=g) * (1.0 / (3 * c ** 0.5))).half().float()  # OIHW
-    bias = torch.randn(c, device="cuda", generator=g)
-    res = torch.randn(n_boards, c, 10, 9, device="cuda", generator=g).half().float() if residual else None
-    xs = _strip_from_nchw(x)
-    ws = w.permute(2, 3, 0, 1).reshape(9, c, c).contiguous().half()          # [tap][c_out][c_in]
-    rs = _strip_from_nchw(res) if residual else None
-    out = torch.full((n_boards * 11, 9, c), float("nan"), device="cuda", dtype=torch.half)
-    cuda_lib.call("cz_igemm_conv3x3", _p(xs), _p(ws), _p(bias), _p(rs), _p(out), n_boards, c, int(relu), _stream())
-    torch.cuda.synchronize()
-    ref, scale = _conv_ref_and_scale(x, w, bias, res, relu)
-    got = _nchw_from_strip(out, n_boards, c)
-    sep = out.reshape(n_boards, 11, 9, c)[:, 10]
-    assert (sep == 0).all()                                   # separator rows stay zero
-    nc.check_close(got, ref, scale, "fp16", what="igemm conv3x3 (strip)")     # one fp16 rounding + fp32 accumulation
-
-
 @pytest.mark.parametrize("n_boards,c,residual,relu", [(1, 128, False, True), (5, 256, True, True), (29, 128, True, False),
                                                        (64, 256, False, False), (200, 192, True, True), (3, 64, True, True),
                                                        (1000, 256, True, True)])

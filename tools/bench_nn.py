@@ -33,16 +33,6 @@ def time_it(fn, iters=10, warm=3):
 def main():
     lib = get_lib()
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    for c, nb in ((256, 8192), (256, 1024), (128, 2048), (128, 8192)):
-        x = torch.zeros(nb * 11, 9, c, device="cuda", dtype=torch.half)
-        x.view(nb, 11, 9, c)[:, :10] = torch.randn(nb, 10, 9, c, device="cuda").half()
-        w = (torch.randn(9, c, c, device="cuda") * 0.02).half()
-        b = torch.zeros(c, device="cuda")
-        y = torch.empty_like(x)
-        ms = time_it(lambda: lib.call("cz_igemm_conv3x3", p(x), p(w), p(b), p(x), p(y), nb, c, 1, st))
-        useful = 2.0 * nb * 90 * 9 * c * c
-        issued = 2.0 * ((nb * 11 + 13) // 14) * 128 * 9 * c * c
-        print(f"conv3x3 C={c} boards={nb}: {ms:.3f} ms  useful {useful / ms / 1e9:.1f} TFLOP/s  issued {issued / ms / 1e9:.1f} TFLOP/s")
     # the product kernel: wgmma conv on dense activations (im2col TMA), without / with the fp16 skip stream
     for c, nb in ((256, 8192), (256, 4096), (128, 2048), (128, 8192), (192, 4096)):
         x = torch.randn(nb, 10, 9, c, device="cuda").half()

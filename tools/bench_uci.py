@@ -1,8 +1,7 @@
 """Single-game latency path: one `CChessPlayer(uci=True)` on the built-in network answering `go depth 8` (= 800 simulations,
 uci.py:293-327 -> player.py:160-161), the way the reference's UCI front end drives its player.  Prints the wall time of the
 search, simulations/s and the `nps` figure computed with the REFERENCE'S formula, nps = int(depth * 100 / duration) * 1000
-(agent/player.py:446-447), for the device-driven loop in both forms (CZ_SEARCH_LOOP=while, the default: one graph launch per
-slice of the search; =graph: three sub-graphs per iteration and a polled flag) and the round-1 host-driven loop (=host).
+(agent/player.py:446-447).  Each slice of the search is one WHILE-graph launch of the device-driven loop.
 
     python tools/bench_uci.py [filters blocks] [depth] [search_threads]
 Weights: the reference's trained 192x10 network when CZ_WEIGHTS names an .npz of it (tools/convert_h5.py writes one), seeded
@@ -21,14 +20,15 @@ import torch         # noqa: E402
 
 
 def run(loop, filters, blocks, depth, k, weights):
-    os.environ["CZ_SEARCH_LOOP"] = loop
+    """`loop` names the search loop form to time; "while" is the only one there is."""
+    if loop != "while":
+        raise ValueError(f"search loop {loop!r}: the engine has one loop form, 'while'")
     from cczero_b200.player import CChessPlayer
     from cczero_b200.env import INIT_STATE
     play = SimpleNamespace(simulation_num_per_move=800, search_threads=k, c_puct=1.5, noise_eps=0.15, dirichlet_alpha=0.2,
                            tau_decay_rate=0.9, virtual_loss=3, resign_threshold=-0.98, min_resign_turn=40, max_game_length=100)
     cfg = SimpleNamespace(play=play, model=SimpleNamespace(cnn_filter_num=filters, res_layer_num=blocks, value_fc_size=256, input_depth=14))
     p = CChessPlayer(cfg, uci=True, weights=weights, exact_noise=False, infinite_capacity=20000)
-    os.environ.pop("CZ_SEARCH_LOOP", None)
     p.info_stream = io.StringIO()
     out = []
     state = INIT_STATE
@@ -64,9 +64,8 @@ def main():
     k = int(sys.argv[4]) if len(sys.argv) > 4 else 10      # configs/distribute.py: search_threads = 10
     weights, src = load_weights(filters, blocks)
     res = {"net": f"{filters}x{blocks}", "weights": src, "go": f"depth {depth} ({depth * 100} simulations), search_threads {k}"}
-    for loop in os.environ.get("UCI_LOOPS", "while,graph,host").split(","):      # one WHILE-graph launch per slice (default) | three sub-graphs per iteration | round-1 host loop
-        runs, info = run(loop, filters, blocks, depth, k, weights)
-        res[loop] = {"best": min(runs[1:], key=lambda r: r["seconds"]), "runs": runs, "last_info_line": info}
+    runs, info = run("while", filters, blocks, depth, k, weights)
+    res["while"] = {"best": min(runs[1:], key=lambda r: r["seconds"]), "runs": runs, "last_info_line": info}
     print(json.dumps(res))
 
 
