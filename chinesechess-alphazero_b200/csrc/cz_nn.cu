@@ -27,12 +27,6 @@
 
 namespace cznn {
 
-#define CZ_CUDA(x)                                                                           \
-  do {                                                                                       \
-    cudaError_t e__ = (x);                                                                   \
-    if (e__ != cudaSuccess) return cz_fail(CZ_ERR_CUDA, "%s: %s", #x, cudaGetErrorString(e__)); \
-  } while (0)
-
 constexpr int kLabels = CZ_N_LABELS;
 // Head widths are a property of the weight file: agent/model.py:47-61 builds 4 policy / 2 value channels, the older configs shipped
 // under data/model/ (model_128f.json, model_256f.json: 2 / 4; model_128_l1_config.json: 32 / 4) are served too.
@@ -126,13 +120,7 @@ int num_sms() {
 }
 
 // Programmatic dependent launch: a conv's CTAs may become resident and run their prologue (barrier init, tensor-map prefetch)
-// while the previous kernel of the stream is still running; griddepcontrol.wait in the kernel orders the data.  CZ_PDL=0
-// launches the plain way.
-static bool use_pdl() {
-  static int pdl = -1;
-  if (pdl < 0) { const char* e = getenv("CZ_PDL"); pdl = (e && e[0] == '0') ? 0 : 1; }
-  return pdl == 1;
-}
+// while the previous kernel of the stream is still running; griddepcontrol.wait in the kernel orders the data.
 template <int N_TILE>
 static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut, const igemm::Args& a, cudaStream_t st) {
   using C = igemm::Cfg<N_TILE>;
@@ -144,18 +132,14 @@ static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const 
   const int tiles = a.m_tiles * a.n_tiles;
   if (tiles <= 0) return 0;
   const int grid = tiles < num_sms() ? tiles : num_sms();
-  if (use_pdl()) {
-    cudaLaunchConfig_t lc;
-    memset(&lc, 0, sizeof(lc));
-    lc.gridDim = dim3(grid); lc.blockDim = dim3(igemm::kThreads); lc.dynamicSmemBytes = C::kSmemBytes; lc.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    lc.attrs = at; lc.numAttrs = 1;
-    CZ_CUDA(cudaLaunchKernelEx(&lc, igemm::k_igemm<N_TILE>, tmA, tmB, tmOut, a));
-  } else {
-    igemm::k_igemm<N_TILE><<<grid, igemm::kThreads, C::kSmemBytes, st>>>(tmA, tmB, tmOut, a);
-  }
+  cudaLaunchConfig_t lc;
+  memset(&lc, 0, sizeof(lc));
+  lc.gridDim = dim3(grid); lc.blockDim = dim3(igemm::kThreads); lc.dynamicSmemBytes = C::kSmemBytes; lc.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  lc.attrs = at; lc.numAttrs = 1;
+  CZ_CUDA(cudaLaunchKernelEx(&lc, igemm::k_igemm<N_TILE>, tmA, tmB, tmOut, a));
   CZ_CUDA(cudaGetLastError());
   return 0;
 }
@@ -174,11 +158,9 @@ int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, con
   return cz_fail(CZ_ERR_UNSUPPORTED, "igemm: unsupported N tile %d (filters must be 64/128/192/256)", n_tile);
 }
 // Small batches (one game's leaves: the UCI / play_games latency path): 64-column tiles, m_tiles x C/64 work items, as long as
-// they fit one wave of CTAs.  The weight map then has 64-row boxes (map_w_64).  CZ_NSPLIT=0 turns it off.
+// they fit one wave of CTAs.  The weight map then has 64-row boxes (NetWeights::map_w_64).
 static bool use_n_split(int n_boards, int c) {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("CZ_NSPLIT"); on = (e && e[0] == '0') ? 0 : 1; }
-  if (!on || c <= 64) return false;
+  if (c <= 64) return false;
   const int m_tiles = (n_boards * 90 + igemm::kTileM - 1) / igemm::kTileM;
   return m_tiles * (c / 64) <= num_sms();
 }
@@ -488,33 +470,25 @@ __global__ void k_copy_pad(const float* src, float* dst, int n_src, int n_dst) {
 }
 
 // ------------------------------------------------------------------------------------------------
-struct Carver {
-  uint8_t* base; size_t off, cap;
-  void* take(size_t bytes) {
-    off = (off + 1023) & ~(size_t)1023;
-    void* p = base ? base + off : nullptr;
-    off += bytes;
-    return p;
-  }
-};
-
-// One network's folded weights (the arena holds two: best vs next generation, worker/evaluator.py:28-82).
+// One network's folded weights and their tensor maps (the arena holds two: best vs next generation,
+// worker/evaluator.py:28-82).  nn_create fixes the buffers and maps for the runtime's lifetime: the search's captured graphs
+// hold them by value, so cz_nn_set_weights may reload a network without a re-capture.
 struct NetWeights {
   __half* w_first; float* shift_first;
-  __half* w_conv;  float* shift_conv;
+  __half* w_conv;  float* shift_conv;      // [2*blocks][9*C*C], [2*blocks][C]
   float *wh, *shifth, *wv1, *bv1, *wv2, *bv2;
   __half* w_pol; float* b_pol;
   CUtensorMap map_wpol;
-  std::vector<CUtensorMap> map_w, map_w_64;
-  bool ready;
+  std::vector<CUtensorMap> map_w;
+  std::vector<CUtensorMap> map_w_64;       // box rows = 64: 64-column tiles of the small-batch launches (use_n_split)
+  bool ready;                              // weights set (nn_set_weights)
 };
 
 struct NnRuntime {
   int filters, blocks, value_fc, max_batch;
   int pol_c, val_c, pol_k1;               // head widths (policy / value conv channels) and the padded policy feature count
-  NetWeights nets[2]; int n_nets, cur;     // the weight fields below alias nets[cur] (select_net / store_net)
+  NetWeights nets[2]; int n_nets;
   cudaStream_t stream;
-  bool ready;
   uint64_t launches;
   // activations
   __half *x, *t, *y, *pol_feat;
@@ -527,16 +501,8 @@ struct NnRuntime {
   size_t prof_open;                      // event pair opened by nn_prof_begin
   uint8_t* boards_tmp;
   int in_planes;                         // 14, or 28 with use_history (board + history board per position)
-  // weights
-  __half* w_first; float* shift_first;
-  __half* w_conv;  float* shift_conv;      // [2*blocks][9*C*C], [2*blocks][C]
-  float *wh, *shifth, *wv1, *bv1, *wv2, *bv2;
-  __half* w_pol; float* b_pol;
   float* scratch;                            // 2*C floats for BN folding
-  // tensor maps
-  CUtensorMap map_pf, map_wpol;
-  std::vector<CUtensorMap> map_w;
-  std::vector<CUtensorMap> map_w_64;     // box rows = 64: 64-column tiles of the small-batch launches (use_n_split)
+  CUtensorMap map_pf;                    // policy GEMM operand (pol_feat)
   bool fp32_skip;                        // keep the residual (skip) stream in fp32: halves the value error of deep nets, ~+30 % time
   CUtensorMap imap_x, imap_t, imap_y;    // im2col maps of the three activation buffers
   CUtensorMap emap_t;                    // conv1's output buffer as the staged conv epilogue stores it
@@ -547,24 +513,6 @@ struct NnRuntime {
   std::vector<double> ev_flops;       // algorithmic flops bracketed by pair i
   double prof_ms, prof_flops; uint64_t prof_launches;
 };
-
-static void store_net(NnRuntime* r, int k) {
-  NetWeights& n = r->nets[k];
-  n.w_first = r->w_first; n.shift_first = r->shift_first; n.w_conv = r->w_conv; n.shift_conv = r->shift_conv;
-  n.wh = r->wh; n.shifth = r->shifth; n.wv1 = r->wv1; n.bv1 = r->bv1; n.wv2 = r->wv2; n.bv2 = r->bv2;
-  n.w_pol = r->w_pol; n.b_pol = r->b_pol; n.map_wpol = r->map_wpol; n.map_w = r->map_w; n.map_w_64 = r->map_w_64;
-  n.ready = r->ready;
-}
-static void select_net(NnRuntime* r, int k) {
-  if (r->cur == k) return;
-  store_net(r, r->cur);
-  const NetWeights& n = r->nets[k];
-  r->w_first = n.w_first; r->shift_first = n.shift_first; r->w_conv = n.w_conv; r->shift_conv = n.shift_conv;
-  r->wh = n.wh; r->shifth = n.shifth; r->wv1 = n.wv1; r->bv1 = n.bv1; r->wv2 = n.wv2; r->bv2 = n.bv2;
-  r->w_pol = n.w_pol; r->b_pol = n.b_pol; r->map_wpol = n.map_wpol; r->map_w = n.map_w; r->map_w_64 = n.map_w_64;
-  r->ready = n.ready;
-  r->cur = k;
-}
 
 static void prof_collect(NnRuntime* r) {
   for (size_t i = 0; i + 1 < r->ev_used; i += 2) {
@@ -589,25 +537,21 @@ static void layout(NnRuntime* r, Carver& cv) {
   r->stats = (float2*)cv.take((size_t)r->max_batch * (kPolN / 256) * sizeof(float2));
   r->n_scalar = (int*)cv.take(64);
   r->boards_tmp = (uint8_t*)cv.take((size_t)r->max_batch * 2 * CZ_BOARD_STRIDE);
-  for (int net = 0; net < r->n_nets; ++net) {
-  r->w_first = (__half*)cv.take((size_t)25 * 28 * c * sizeof(__half));
-  r->shift_first = (float*)cv.take(c * sizeof(float));
-  r->w_conv = (__half*)cv.take((size_t)2 * r->blocks * 9 * c * c * sizeof(__half));
-  r->shift_conv = (float*)cv.take((size_t)2 * r->blocks * c * sizeof(float));
-  r->wh = (float*)cv.take((size_t)(r->pol_c + r->val_c) * c * sizeof(float));
-  r->shifth = (float*)cv.take((size_t)(r->pol_c + r->val_c + 4) * sizeof(float));
-  r->wv1 = (float*)cv.take((size_t)r->val_c * 90 * r->value_fc * sizeof(float));
-  r->bv1 = (float*)cv.take(r->value_fc * sizeof(float));
-  r->wv2 = (float*)cv.take(r->value_fc * sizeof(float));
-  r->bv2 = (float*)cv.take(4 * sizeof(float));
-  r->w_pol = (__half*)cv.take((size_t)kPolN * 3 * r->pol_k1 * sizeof(__half));
-  r->b_pol = (float*)cv.take(kPolN * sizeof(float));
-  r->ready = false;
-  r->cur = net;
-  store_net(r, net);
+  for (int k = 0; k < r->n_nets; ++k) {
+    NetWeights& w = r->nets[k];
+    w.w_first = (__half*)cv.take((size_t)25 * 28 * c * sizeof(__half));
+    w.shift_first = (float*)cv.take(c * sizeof(float));
+    w.w_conv = (__half*)cv.take((size_t)2 * r->blocks * 9 * c * c * sizeof(__half));
+    w.shift_conv = (float*)cv.take((size_t)2 * r->blocks * c * sizeof(float));
+    w.wh = (float*)cv.take((size_t)(r->pol_c + r->val_c) * c * sizeof(float));
+    w.shifth = (float*)cv.take((size_t)(r->pol_c + r->val_c + 4) * sizeof(float));
+    w.wv1 = (float*)cv.take((size_t)r->val_c * 90 * r->value_fc * sizeof(float));
+    w.bv1 = (float*)cv.take(r->value_fc * sizeof(float));
+    w.wv2 = (float*)cv.take(r->value_fc * sizeof(float));
+    w.bv2 = (float*)cv.take(4 * sizeof(float));
+    w.w_pol = (__half*)cv.take((size_t)kPolN * 3 * r->pol_k1 * sizeof(__half));
+    w.b_pol = (float*)cv.take(kPolN * sizeof(float));
   }
-  if (r->n_nets > 1) { r->cur = r->n_nets - 1; select_net(r, 0); }
-  r->cur = 0;
   r->scratch = (float*)cv.take((size_t)(2 * 256 + 2 * kMaxHeadOut) * sizeof(float));
 }
 
@@ -617,9 +561,9 @@ static void set_heads(NnRuntime* r, int pol_c, int val_c) {
 }
 size_t nn_workspace_bytes(int filters, int blocks, int value_fc, int max_batch, int n_nets, int pol_c, int val_c) {
   NnRuntime tmp;
-  tmp.filters = filters; tmp.blocks = blocks; tmp.value_fc = value_fc; tmp.max_batch = max_batch; tmp.n_nets = n_nets; tmp.cur = 0;
+  tmp.filters = filters; tmp.blocks = blocks; tmp.value_fc = value_fc; tmp.max_batch = max_batch; tmp.n_nets = n_nets;
   set_heads(&tmp, pol_c, val_c);
-  Carver cv{nullptr, 0, 0};
+  Carver cv{nullptr, 0};
   layout(&tmp, cv);
   return cv.off + 4096;
 }
@@ -637,16 +581,15 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
   NnRuntime* r = new NnRuntime();
   set_heads(r, pol_c, val_c);
   r->heads_attr = false;
-  r->filters = filters; r->blocks = blocks; r->value_fc = value_fc; r->max_batch = max_batch; r->n_nets = n_nets; r->cur = 0;
-  r->stream = (cudaStream_t)stream; r->ready = false; r->launches = 0;
+  r->filters = filters; r->blocks = blocks; r->value_fc = value_fc; r->max_batch = max_batch; r->n_nets = n_nets;
+  r->stream = (cudaStream_t)stream; r->launches = 0;
   r->in_planes = in_planes == 28 ? 28 : 14;
   // 0 = auto (fp32 skip stream for towers of 10 blocks and more, where fp16 rounding of the skip stream pushes the outputs
   // past 1e-3: value 1.1e-3 .. 1.5e-3 at 20 random-init blocks vs <= 6e-4 with fp32; policy 1.6e-3 vs 9.8e-4 on the
   // reference's trained 192x10 net), 1 = always, 2 = never
   r->fp32_skip = fp32_skip_mode == 1 || (fp32_skip_mode == 0 && blocks >= 10);
-  { const char* e = getenv("CZ_FP32_SKIP"); if (e && e[0] == '1') r->fp32_skip = true; if (e && e[0] == '0') r->fp32_skip = false; }
   r->profile = false; r->ev_used = 0; r->prof_ms = 0; r->prof_flops = 0; r->prof_launches = 0; r->capturing = false;
-  Carver cv{(uint8_t*)workspace, 0, bytes};
+  Carver cv{(uint8_t*)workspace, 0};
   layout(r, cv);
   const int c = filters;
   int rc = 0;
@@ -655,16 +598,16 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
   rc |= make_map_im2col(&r->imap_y, r->y, c, max_batch);
   rc |= make_map_epi(&r->emap_t, r->t, c, (long long)max_batch * 90);
   rc |= make_map_2d(&r->map_pf, r->pol_feat, 3 * r->pol_k1, (long long)max_batch + 128, 128);
-  for (int net = n_nets - 1; net >= 0; --net) {
-    select_net(r, net);
-    rc |= make_map_2d(&r->map_wpol, r->w_pol, 3 * r->pol_k1, kPolN, 256);
-    r->map_w.resize(2 * blocks);
-    r->map_w_64.resize(2 * blocks);
+  for (int k = 0; k < n_nets; ++k) {
+    NetWeights& w = r->nets[k];
+    w.ready = false;
+    rc |= make_map_2d(&w.map_wpol, w.w_pol, 3 * r->pol_k1, kPolN, 256);
+    w.map_w.resize(2 * blocks);
+    w.map_w_64.resize(2 * blocks);
     for (int i = 0; i < 2 * blocks; ++i) {
-      rc |= make_map_2d(&r->map_w[i], r->w_conv + (size_t)i * 9 * c * c, c, 9LL * c, c);
-      rc |= make_map_2d(&r->map_w_64[i], r->w_conv + (size_t)i * 9 * c * c, c, 9LL * c, 64);
+      rc |= make_map_2d(&w.map_w[i], w.w_conv + (size_t)i * 9 * c * c, c, 9LL * c, c);
+      rc |= make_map_2d(&w.map_w_64[i], w.w_conv + (size_t)i * 9 * c * c, c, 9LL * c, 64);
     }
-    store_net(r, net);
   }
   if (rc) { delete r; return nullptr; }
   // the last, partial M tile of a conv or of the policy GEMM loads rows past the batch: they start as zeros, not as whatever
@@ -696,38 +639,40 @@ int nn_profile_read(NnRuntime* r, double* ms, uint64_t* launches, double* flops)
 bool nn_ready(const NnRuntime* r) {
   if (!r) return false;
   for (int k = 0; k < r->n_nets; ++k)
-    if (!(k == r->cur ? r->ready : r->nets[k].ready)) return false;
+    if (!r->nets[k].ready) return false;
   return true;
+}
+// Network `net` of r if its weights are set; null (and cz_last_error says why) otherwise.
+static const NetWeights* ready_net(NnRuntime* r, int net) {
+  if (!r || net < 0 || net >= r->n_nets) { cz_fail(CZ_ERR_STATE, "no such network"); return nullptr; }
+  if (!r->nets[net].ready) { cz_fail(CZ_ERR_STATE, "network weights not set (cz_nn_set_weights)"); return nullptr; }
+  return &r->nets[net];
 }
 uint64_t nn_launches(const NnRuntime* r) { return r ? r->launches : 0; }
 
 // ---- weights -----------------------------------------------------------------------------------
-struct WeightSet {
-  const cz_tensor_desc* d; int n;
-  // find "<layer prefix>...<'/'><weight>" ; Keras appends "-<k>-<f>" to conv layer names and ":0" to weights
-  const cz_tensor_desc* find(const std::string& layer, const std::string& weight) const {
-    for (int i = 0; i < n; ++i) {
-      std::string nm = d[i].name ? d[i].name : "";
-      const size_t slash = nm.find('/');
-      if (slash == std::string::npos) continue;
-      std::string l = nm.substr(0, slash), w = nm.substr(slash + 1);
-      const size_t colon = w.find(':');
-      if (colon != std::string::npos) w = w.substr(0, colon);
-      const size_t s2 = w.find('/');            // "layer/layer/kernel" style
-      if (s2 != std::string::npos) w = w.substr(s2 + 1);
-      if (w != weight) continue;
-      if (l == layer || (l.size() > layer.size() && l.compare(0, layer.size(), layer) == 0 && l[layer.size()] == '-')) return &d[i];
-    }
-    return nullptr;
+const cz_tensor_desc* find_keras_tensor(const cz_tensor_desc* descs, int n, const std::string& layer, const std::string& weight) {
+  for (int i = 0; i < n; ++i) {
+    std::string nm = descs[i].name ? descs[i].name : "";
+    const size_t slash = nm.find('/');
+    if (slash == std::string::npos) continue;
+    std::string l = nm.substr(0, slash), w = nm.substr(slash + 1);
+    const size_t colon = w.find(':');
+    if (colon != std::string::npos) w = w.substr(0, colon);
+    const size_t s2 = w.find('/');            // "layer/layer/kernel" style
+    if (s2 != std::string::npos) w = w.substr(s2 + 1);
+    if (w != weight) continue;
+    if (l == layer || (l.size() > layer.size() && l.compare(0, layer.size(), layer) == 0 && l[layer.size()] == '-')) return &descs[i];
   }
-};
+  return nullptr;
+}
 
 #define NEED(var, layer, weight, count)                                                                      \
-  const cz_tensor_desc* var = ws.find(layer, weight);                                                        \
+  const cz_tensor_desc* var = find_keras_tensor(descs, n_descs, layer, weight);                              \
   if (!var || var->numel != (long long)(count))                                                              \
     return cz_fail(CZ_ERR_ARG, "cz_nn_set_weights: missing or mis-sized tensor %s/%s (want %lld)", std::string(layer).c_str(), weight, (long long)(count));
 
-static int fold_bn(NnRuntime* r, const WeightSet& ws, const std::string& layer, int c, float* scale, float* shift) {
+static int fold_bn(NnRuntime* r, const cz_tensor_desc* descs, int n_descs, const std::string& layer, int c, float* scale, float* shift) {
   NEED(g, layer, "gamma", c);
   NEED(b, layer, "beta", c);
   NEED(m, layer, "moving_mean", c);
@@ -738,19 +683,18 @@ static int fold_bn(NnRuntime* r, const WeightSet& ws, const std::string& layer, 
   return 0;
 }
 
-int nn_set_weights(NnRuntime* r, int net, const cz_tensor_desc* descs, int n) {
+int nn_set_weights(NnRuntime* r, int net, const cz_tensor_desc* descs, int n_descs) {
   if (!r) return cz_fail(CZ_ERR_STATE, "cz_nn_set_weights: engine was created without a network (nn_filters = 0)");
   if (net < 0 || net >= r->n_nets) return cz_fail(CZ_ERR_ARG, "cz_nn_set_weights: network %d of %d", net, r->n_nets);
-  select_net(r, net);
-  WeightSet ws{descs, n};
+  NetWeights& w = r->nets[net];
   const int c = r->filters;
   cudaStream_t st = r->stream;
   float* scale = r->scratch;
   {
     NEED(k, "input_conv", "kernel", 25LL * r->in_planes * c);
-    if (fold_bn(r, ws, "input_batchnorm", c, scale, r->shift_first)) return CZ_ERR_ARG;
+    if (fold_bn(r, descs, n_descs, "input_batchnorm", c, scale, w.shift_first)) return CZ_ERR_ARG;
     const long long nn = 25LL * r->in_planes * c;
-    k_prep_hwio<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>((const float*)k->dev, scale, r->w_first, nn, c);
+    k_prep_hwio<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>((const float*)k->dev, scale, w.w_first, nn, c);
   }
   for (int i = 0; i < r->blocks; ++i) {
     for (int j = 0; j < 2; ++j) {
@@ -758,27 +702,27 @@ int nn_set_weights(NnRuntime* r, int net, const cz_tensor_desc* descs, int n) {
       const std::string bn = "res" + std::to_string(i + 1) + "_batchnorm" + std::to_string(j + 1);
       NEED(k, conv, "kernel", 9LL * c * c);
       const int li = 2 * i + j;
-      if (fold_bn(r, ws, bn, c, scale, r->shift_conv + (size_t)li * c)) return CZ_ERR_ARG;
+      if (fold_bn(r, descs, n_descs, bn, c, scale, w.shift_conv + (size_t)li * c)) return CZ_ERR_ARG;
       const long long nn = 9LL * c * c;
-      k_prep_conv3<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>((const float*)k->dev, scale, r->w_conv + (size_t)li * nn, c);
+      k_prep_conv3<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>((const float*)k->dev, scale, w.w_conv + (size_t)li * nn, c);
     }
   }
   {
     const int pc = r->pol_c, vc = r->val_c;
     NEED(kp, "policy_conv", "kernel", (long long)pc * c);
-    if (fold_bn(r, ws, "policy_batchnorm", pc, scale, r->shifth)) return CZ_ERR_ARG;
-    k_prep_1x1<<<(pc * c + 255) / 256, 256, 0, st>>>((const float*)kp->dev, scale, r->wh, c, pc);
+    if (fold_bn(r, descs, n_descs, "policy_batchnorm", pc, scale, w.shifth)) return CZ_ERR_ARG;
+    k_prep_1x1<<<(pc * c + 255) / 256, 256, 0, st>>>((const float*)kp->dev, scale, w.wh, c, pc);
     NEED(kv, "value_conv", "kernel", (long long)vc * c);
     float* scale_v = r->scratch + 2 * 256 + kMaxHeadOut;     // k_bn_fold of the policy head above may still be reading `scale`
-    if (fold_bn(r, ws, "value_batchnorm", vc, scale_v, r->shifth + pc)) return CZ_ERR_ARG;
-    k_prep_1x1<<<(vc * c + 255) / 256, 256, 0, st>>>((const float*)kv->dev, scale_v, r->wh + (size_t)pc * c, c, vc);
+    if (fold_bn(r, descs, n_descs, "value_batchnorm", vc, scale_v, w.shifth + pc)) return CZ_ERR_ARG;
+    k_prep_1x1<<<(vc * c + 255) / 256, 256, 0, st>>>((const float*)kv->dev, scale_v, w.wh + (size_t)pc * c, c, vc);
   }
   {
     NEED(k, "policy_out", "kernel", (long long)r->pol_c * 90 * kLabels);
     NEED(b, "policy_out", "bias", kLabels);
     const long long nn = (long long)kPolN * r->pol_k1;
-    k_prep_policy<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>((const float*)k->dev, r->w_pol, r->pol_c * 90, r->pol_k1);
-    k_copy_pad<<<(kPolN + 255) / 256, 256, 0, st>>>((const float*)b->dev, r->b_pol, kLabels, kPolN);
+    k_prep_policy<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>((const float*)k->dev, w.w_pol, r->pol_c * 90, r->pol_k1);
+    k_copy_pad<<<(kPolN + 255) / 256, 256, 0, st>>>((const float*)b->dev, w.b_pol, kLabels, kPolN);
   }
   {
     const int h = r->value_fc;
@@ -786,15 +730,15 @@ int nn_set_weights(NnRuntime* r, int net, const cz_tensor_desc* descs, int n) {
     NEED(b1, "value_dense", "bias", h);
     NEED(k2, "value_out", "kernel", h);
     NEED(b2, "value_out", "bias", 1);
-    CZ_CUDA(cudaMemcpyAsync(r->wv1, k1->dev, (size_t)r->val_c * 90 * h * 4, cudaMemcpyDeviceToDevice, st));
-    CZ_CUDA(cudaMemcpyAsync(r->bv1, b1->dev, (size_t)h * 4, cudaMemcpyDeviceToDevice, st));
-    CZ_CUDA(cudaMemcpyAsync(r->wv2, k2->dev, (size_t)h * 4, cudaMemcpyDeviceToDevice, st));
-    CZ_CUDA(cudaMemcpyAsync(r->bv2, b2->dev, 4, cudaMemcpyDeviceToDevice, st));
+    CZ_CUDA(cudaMemcpyAsync(w.wv1, k1->dev, (size_t)r->val_c * 90 * h * 4, cudaMemcpyDeviceToDevice, st));
+    CZ_CUDA(cudaMemcpyAsync(w.bv1, b1->dev, (size_t)h * 4, cudaMemcpyDeviceToDevice, st));
+    CZ_CUDA(cudaMemcpyAsync(w.wv2, k2->dev, (size_t)h * 4, cudaMemcpyDeviceToDevice, st));
+    CZ_CUDA(cudaMemcpyAsync(w.bv2, b2->dev, 4, cudaMemcpyDeviceToDevice, st));
   }
   r->launches += 6 + 2 * r->blocks;
   CZ_CUDA(cudaGetLastError());
   CZ_CUDA(cudaStreamSynchronize(st));
-  r->ready = true;
+  w.ready = true;
   return 0;
 }
 
@@ -810,18 +754,18 @@ static int conv_first_threads(int c) {                    // (c/2) channel pairs
   while (pairs * g < 96) ++g;                             // phase 1 needs 90 threads
   return pairs * g;
 }
-static int fw_first(NnRuntime* r, const uint8_t* boards, int n, const int* n_dev) {
+static int fw_first(NnRuntime* r, const NetWeights& w, const uint8_t* boards, int n, const int* n_dev) {
   const int c = r->filters;
   const bool s32 = r->fp32_skip;
   int slices = (2 * num_sms() + n - 1) / n;                // >= 2 CTAs per SM in flight; big batches: one CTA per position
   if (slices > 15) slices = 15;
-  k_conv_first<<<dim3(n, slices), conv_first_threads(c), 0, r->stream>>>(boards, r->w_first, r->shift_first, r->x, s32 ? r->x32 : nullptr, c,
+  k_conv_first<<<dim3(n, slices), conv_first_threads(c), 0, r->stream>>>(boards, w.w_first, w.shift_first, r->x, s32 ? r->x32 : nullptr, c,
                                                             r->in_planes, (r->in_planes / 14) * CZ_BOARD_STRIDE, n_dev);
   r->launches++;
   CZ_CUDA(cudaGetLastError());
   return 0;
 }
-static int fw_tower(NnRuntime* r, int n, const int* n_dev) {
+static int fw_tower(NnRuntime* r, const NetWeights& w, int n, const int* n_dev) {
   const int c = r->filters;
   cudaStream_t st = r->stream;
   float *x32 = r->fp32_skip ? r->x32 : nullptr, *y32 = r->fp32_skip ? r->y32 : nullptr;
@@ -829,11 +773,11 @@ static int fw_tower(NnRuntime* r, int n, const int* n_dev) {
   __half *x = r->x, *y = r->y;
   const bool split = use_n_split(n, c);
   const int nt = split ? 64 : c;
-  const std::vector<CUtensorMap>& wm = split ? r->map_w_64 : r->map_w;
+  const std::vector<CUtensorMap>& wm = split ? w.map_w_64 : w.map_w;
   for (int i = 0; i < r->blocks; ++i) {
     // conv1: x -> t (no skip);  conv2: t (+ skip x or x32) -> y (+ y32)
-    igemm::Args d1 = conv_args(n, c, r->shift_conv + (size_t)(2 * i) * c, nullptr, r->t, 1);
-    igemm::Args d2 = conv_args(n, c, r->shift_conv + (size_t)(2 * i + 1) * c, x, y, 1);
+    igemm::Args d1 = conv_args(n, c, w.shift_conv + (size_t)(2 * i) * c, nullptr, r->t, 1);
+    igemm::Args d2 = conv_args(n, c, w.shift_conv + (size_t)(2 * i + 1) * c, x, y, 1);
     d1.n_dev = d2.n_dev = n_dev;
     d2.residual32 = x32; d2.out32 = y32;
     d1.n_tiles = d2.n_tiles = c / nt;
@@ -844,7 +788,7 @@ static int fw_tower(NnRuntime* r, int n, const int* n_dev) {
   }
   return 0;
 }
-static int fw_heads(NnRuntime* r, int n, const int* n_dev, float* value) {
+static int fw_heads(NnRuntime* r, const NetWeights& w, int n, const int* n_dev, float* value) {
   const int c = r->filters;
   const bool s32 = r->fp32_skip;
   const bool odd = (r->blocks & 1) != 0;                   // the tower ping-pongs x <-> y once per block
@@ -856,11 +800,11 @@ static int fw_heads(NnRuntime* r, int n, const int* n_dev, float* value) {
     r->heads_attr = true;
   }
   const int hp = n <= 2 * num_sms() ? 1 : kHeadPos;       // small batches: a block per position (same arithmetic per position)
-  k_heads<<<(n + hp - 1) / hp, 256, hsm, r->stream>>>(x, x32, c, n_dev, r->pol_c, r->val_c, r->pol_k1, r->wh, r->shifth,
-                                                      r->wv1, r->bv1, r->wv2, r->bv2, r->value_fc, r->pol_feat, value, hp);
-  igemm::Args ap = dense_args(n, kLabels, kPolN, 3 * r->pol_k1, 256, r->b_pol, r->logits, kPolN);
+  k_heads<<<(n + hp - 1) / hp, 256, hsm, r->stream>>>(x, x32, c, n_dev, r->pol_c, r->val_c, r->pol_k1, w.wh, w.shifth,
+                                                      w.wv1, w.bv1, w.wv2, w.bv2, r->value_fc, r->pol_feat, value, hp);
+  igemm::Args ap = dense_args(n, kLabels, kPolN, 3 * r->pol_k1, 256, w.b_pol, r->logits, kPolN);
   ap.n_dev = n_dev; ap.rows_per_unit = 1; ap.row_stats = r->stats;
-  if (launch_igemm(256, r->map_pf, r->map_wpol, ap, r->stream)) return CZ_ERR_CUDA;
+  if (launch_igemm(256, r->map_pf, w.map_wpol, ap, r->stream)) return CZ_ERR_CUDA;
   r->launches += 2;
   CZ_CUDA(cudaGetLastError());
   return 0;
@@ -881,20 +825,20 @@ void nn_prof_end(NnRuntime* r) {
   if (r->prof_open != (size_t)-1) cudaEventRecord(r->ev[r->prof_open + 1], r->stream);
   r->prof_open = (size_t)-1;
 }
-static int forward_tower(NnRuntime* r, const uint8_t* boards, int n_max, const int* n_dev, float* value) {
-  int rc = fw_first(r, boards, n_max, n_dev);
+static int forward_tower(NnRuntime* r, const NetWeights& w, const uint8_t* boards, int n_max, const int* n_dev, float* value) {
+  int rc = fw_first(r, w, boards, n_max, n_dev);
   if (rc) return rc;
   nn_prof_begin(r, 2.0 * 90.0 * 9.0 * r->filters * r->filters * (double)n_max * 2.0 * r->blocks);
-  rc = fw_tower(r, n_max, n_dev);
+  rc = fw_tower(r, w, n_max, n_dev);
   nn_prof_end(r);
   if (rc) return rc;
-  return fw_heads(r, n_max, n_dev, value);
+  return fw_heads(r, w, n_max, n_dev, value);
 }
 
 // host-known batch: the reference-facing predict_on_batch (api.py:62-64) -> the full softmax vector
-static int forward_chunk(NnRuntime* r, const uint8_t* boards, int n, float* policy, float* value) {
+static int forward_chunk(NnRuntime* r, const NetWeights& w, const uint8_t* boards, int n, float* policy, float* value) {
   k_set_int<<<1, 1, 0, r->stream>>>(r->n_scalar, n);
-  const int rc = forward_tower(r, boards, n, r->n_scalar, value);
+  const int rc = forward_tower(r, w, boards, n, r->n_scalar, value);
   if (rc) return rc;
   k_softmax<<<n, 256, 0, r->stream>>>(r->logits, kPolN, r->stats, kPolN / 256, policy);
   r->launches += 2;
@@ -903,26 +847,24 @@ static int forward_chunk(NnRuntime* r, const uint8_t* boards, int n, float* poli
 }
 
 int nn_forward_boards(NnRuntime* r, int net, const uint8_t* boards, int batch, float* policy, float* value) {
-  if (!r || net < 0 || net >= r->n_nets) return cz_fail(CZ_ERR_STATE, "no such network");
-  select_net(r, net);
-  if (!r->ready) return cz_fail(CZ_ERR_STATE, "network weights not set (cz_nn_set_weights)");
+  const NetWeights* w = ready_net(r, net);
+  if (!w) return CZ_ERR_STATE;
   for (int off = 0; off < batch; off += r->max_batch) {
     const int n = batch - off < r->max_batch ? batch - off : r->max_batch;
-    const int rc = forward_chunk(r, boards + (size_t)off * (r->in_planes / 14) * CZ_BOARD_STRIDE, n, policy + (size_t)off * kLabels, value + off);
+    const int rc = forward_chunk(r, *w, boards + (size_t)off * (r->in_planes / 14) * CZ_BOARD_STRIDE, n, policy + (size_t)off * kLabels, value + off);
     if (rc) return rc;
   }
   return 0;
 }
 
 int nn_forward_planes(NnRuntime* r, int net, const float* planes, int batch, float* policy, float* value) {
-  if (!r || net < 0 || net >= r->n_nets) return cz_fail(CZ_ERR_STATE, "no such network");
-  select_net(r, net);
-  if (!r->ready) return cz_fail(CZ_ERR_STATE, "network weights not set (cz_nn_set_weights)");
+  const NetWeights* w = ready_net(r, net);
+  if (!w) return CZ_ERR_STATE;
   for (int off = 0; off < batch; off += r->max_batch) {
     const int n = batch - off < r->max_batch ? batch - off : r->max_batch;
     k_planes_to_boards<<<n, 96, 0, r->stream>>>(planes + (size_t)off * r->in_planes * 90, r->boards_tmp, n, r->in_planes);
     r->launches++;
-    const int rc = forward_chunk(r, r->boards_tmp, n, policy + (size_t)off * kLabels, value + off);
+    const int rc = forward_chunk(r, *w, r->boards_tmp, n, policy + (size_t)off * kLabels, value + off);
     if (rc) return rc;
   }
   return 0;
@@ -932,14 +874,13 @@ int nn_forward_planes(NnRuntime* r, int net, const float* planes, int batch, flo
 // softmax probabilities of the legal moves [n][CZ_MAX_MOVES] out.  Fixed launch shapes: safe to capture into a CUDA graph.
 int nn_forward_leaves(NnRuntime* r, int net, int part, const uint8_t* boards, int n_max, const int* n_dev, const int16_t* labels,
                       const int32_t* label_counts, float* legal_p, float* value) {
-  if (!r || net < 0 || net >= r->n_nets) return cz_fail(CZ_ERR_STATE, "no such network");
+  const NetWeights* w = ready_net(r, net);
+  if (!w) return CZ_ERR_STATE;
   if (n_max > r->max_batch) return cz_fail(CZ_ERR_ARG, "nn_forward_leaves: %d leaves > max batch %d", n_max, r->max_batch);
-  select_net(r, net);
-  if (!r->ready) return cz_fail(CZ_ERR_STATE, "network weights not set (cz_nn_set_weights)");
   int rc = 0;
-  if (part & 1) rc = fw_first(r, boards, n_max, n_dev);
-  if (!rc && (part & 2)) rc = fw_tower(r, n_max, n_dev);
-  if (!rc && (part & 4)) rc = fw_heads(r, n_max, n_dev, value);
+  if (part & 1) rc = fw_first(r, *w, boards, n_max, n_dev);
+  if (!rc && (part & 2)) rc = fw_tower(r, *w, n_max, n_dev);
+  if (!rc && (part & 4)) rc = fw_heads(r, *w, n_max, n_dev, value);
   if (rc) return rc;
   if (part & 4) k_legal_priors<<<(n_max + 3) / 4, 128, 0, r->stream>>>(r->logits, kPolN, r->stats, kPolN / 256, labels, label_counts, n_dev, legal_p);
   if (part & 4) r->launches++;

@@ -27,11 +27,8 @@
 
 namespace cztrain {
 
-#define CZ_CUDA(x)                                                                           \
-  do {                                                                                       \
-    cudaError_t e__ = (x);                                                                   \
-    if (e__ != cudaSuccess) return cz_fail(CZ_ERR_CUDA, "%s: %s", #x, cudaGetErrorString(e__)); \
-  } while (0)
+using cznn::Carver;
+
 #define CZ_TRY(x)              \
   do {                         \
     const int r__ = (x);       \
@@ -458,16 +455,6 @@ __global__ void k_fill(float* p, long long n, float v) {
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-struct Carver {
-  uint8_t* base; size_t off;
-  void* take(size_t bytes) {
-    off = (off + 1023) & ~(size_t)1023;
-    void* p = base ? base + off : nullptr;
-    off += bytes;
-    return p;
-  }
-};
-
 struct Param {
   std::string layer, weight;   // Keras layer prefix ("res3_conv1") and weight ("kernel")
   long long numel;
@@ -480,18 +467,6 @@ struct Bn {
   float* z;                          // pre-BN input [P][C]; the backward writes dz over it
   float *mean, *var, *rstd;          // batch statistics of the last step
 };
-
-static bool layer_match(const std::string& name, const std::string& layer, const std::string& weight) {
-  const size_t slash = name.find('/');
-  if (slash == std::string::npos) return false;
-  std::string l = name.substr(0, slash), w = name.substr(slash + 1);
-  const size_t colon = w.find(':');
-  if (colon != std::string::npos) w = w.substr(0, colon);
-  const size_t s2 = w.find('/');
-  if (s2 != std::string::npos) w = w.substr(s2 + 1);
-  if (w != weight) return false;
-  return l == layer || (l.size() > layer.size() && l.compare(0, layer.size(), layer) == 0 && l[layer.size()] == '-');
-}
 
 struct Trainer {
   cz_train_config cfg;
@@ -904,9 +879,7 @@ int cz_train_create(const cz_train_config* cfg, void* workspace, uint64_t bytes,
 void cz_train_destroy(cz_trainer* h) { delete h; }
 
 static const cz_tensor_desc* find_desc(const cz_tensor_desc* d, int n, const Param& q) {
-  for (int i = 0; i < n; ++i)
-    if (d[i].name && layer_match(d[i].name, q.layer, q.weight)) return &d[i];
-  return nullptr;
+  return cznn::find_keras_tensor(d, n, q.layer, q.weight);
 }
 
 int cz_train_set_params(cz_trainer* h, const cz_tensor_desc* params, int32_t n, const cz_tensor_desc* velocity, int32_t nv) {
@@ -990,8 +963,9 @@ int cz_train_adam_iterations(cz_trainer* h, int64_t* out) {
 int cz_train_read_grad(cz_trainer* h, const char* name, void* dst, int64_t numel) {
   if (!h || !name || !dst) return cz_fail(CZ_ERR_ARG, "cz_train_read_grad: null argument");
   Trainer* t = &h->t;
+  const cz_tensor_desc named = {name, nullptr, 0};
   for (const Param& q : t->p) {
-    if (!q.train || !layer_match(name, q.layer, q.weight)) continue;
+    if (!q.train || !find_desc(&named, 1, q)) continue;
     if (numel != q.numel) return cz_fail(CZ_ERR_ARG, "cz_train_read_grad: %s has %lld elements, not %lld", name, q.numel, (long long)numel);
     CZ_CUDA(cudaMemcpyAsync(dst, q.g, (size_t)numel * 4, cudaMemcpyDeviceToDevice, t->st));
     CZ_CUDA(cudaStreamSynchronize(t->st));

@@ -1,12 +1,53 @@
 """Drive the REAL reference CChessPlayer (agent/player.py, unmodified) with a deterministic fake network
 over a real multiprocessing.Pipe (SURVEY.md Appendix B).  Build-container only (needs /root/reference)."""
 import threading
+from collections import deque
 from multiprocessing import Pipe
 
 import numpy as np
 
 from . import ref_import
 from .player import fake_eval_from_planes
+
+
+class FifoLock:
+    """Mutual exclusion that hands the lock to the longest waiter on release."""
+
+    def __init__(self):
+        self._guard = threading.Lock()
+        self._waiters = deque()
+        self._held = False
+
+    def __enter__(self):
+        with self._guard:
+            if not self._held:
+                self._held = True
+                return self
+            turn = threading.Lock()
+            turn.acquire()
+            self._waiters.append(turn)
+        turn.acquire()                     # released by the holder's __exit__: the lock is now ours
+        return self
+
+    def __exit__(self, *exc):
+        with self._guard:
+            if self._waiters:
+                self._waiters.popleft().release()
+            else:
+                self._held = False
+
+
+def fair_queue_lock(player):
+    """Give a real player a first-come-first-served prediction-queue lock (call it while the player is idle).
+
+    The player's sender thread holds `q_lock` through its 1 ms sleep whenever the queue is empty and takes it again
+    right after releasing it (agent/player.py:113-123).  threading.Lock is not fair: on a multi-core machine the sender
+    takes it back before the woken search thread that wants to queue a leaf (expand_and_evaluate) runs, so a
+    60-simulation search can take tens of seconds.  With search_threads = 1 the simulations run one after another
+    whatever the timing, so the search itself is unchanged; a threaded player, whose schedule does depend on timing,
+    keeps its own lock."""
+    if player.config.play.search_threads == 1 and not isinstance(player.q_lock, FifoLock):
+        player.q_lock = FifoLock()
 
 
 class FakeNetServer:
@@ -49,6 +90,7 @@ def real_player_moves(states_and_opts, sims, seed, search_threads=1, use_history
     srv = FakeNetServer()
     np.random.seed(seed)
     player = pm.CChessPlayer(cfg, pipes=srv.you, enable_resign=False, use_history=use_history)
+    fair_queue_lock(player)
     out = []
     try:
         for call in states_and_opts:

@@ -18,7 +18,7 @@ from collections import defaultdict
 import numpy as np
 
 from . import ref_import
-from .ref_player_harness import FakeNetServer, make_config
+from .ref_player_harness import FakeNetServer, fair_queue_lock, make_config
 
 
 class _Anything:
@@ -121,6 +121,7 @@ def real_selfplay_game(seed, sims, use_history=False, player_factory=None, **pla
     orig_action = pm.CChessPlayer.action
 
     def spy(self, state, turns, no_act=None, depth=None, infinite=False, hist=None, increase_temp=False):
+        fair_queue_lock(self)
         temps.append(bool(increase_temp))
         return orig_action(self, state, turns, no_act, depth, infinite, hist, increase_temp)
     pm.CChessPlayer.action = spy
@@ -156,6 +157,7 @@ def real_arena_game(seed, idx, sims, player_factory=None, **play):
     orig_action = pm.CChessPlayer.action
 
     def spy(self, state, turns, no_act=None, depth=None, infinite=False, hist=None, increase_temp=False):
+        fair_queue_lock(self)
         if sims is not None:
             self.play_config.simulation_num_per_move = sims
         temps.append(bool(increase_temp))
