@@ -63,8 +63,7 @@ static int load_encode() {
 }
 
 // fp16 NHWC activations [n][10][9][c] read in im2col mode for a 3x3 "same" convolution: the bounding box of base pixels is
-// [-1, dim-2] in w and h (lower corner = -pad, upper corner = pad - (filter-1)), 64 channels x `pixels` (128 for the forward)
-// output pixels per load;
+// [-1, dim-2] in w and h (lower corner = -pad, upper corner = pad - (filter-1)), 64 channels x `pixels` output pixels per load;
 // taps outside the image are zero-filled by the TMA unit, and the pixel column walks across rows and images.
 int make_map_im2col(CUtensorMap* m, const void* base, int c, long long n_images, int pixels) {
   if (load_encode()) return CZ_ERR_CUDA;
@@ -121,12 +120,12 @@ int num_sms() {
 
 // Programmatic dependent launch: a conv's CTAs may become resident and run their prologue (barrier init, tensor-map prefetch)
 // while the previous kernel of the stream is still running; griddepcontrol.wait in the kernel orders the data.
-template <int N_TILE>
+template <int N_TILE, int M_TILE, bool CONV>
 static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmOut, const igemm::Args& a, cudaStream_t st) {
-  using C = igemm::Cfg<N_TILE>;
+  using C = igemm::Cfg<N_TILE, M_TILE, CONV>;
   static bool attr_set = false;
   if (!attr_set) {
-    CZ_CUDA(cudaFuncSetAttribute(igemm::k_igemm<N_TILE>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
+    CZ_CUDA(cudaFuncSetAttribute(igemm::k_igemm<N_TILE, M_TILE, CONV>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
     attr_set = true;
   }
   const int tiles = a.m_tiles * a.n_tiles;
@@ -139,7 +138,7 @@ static int launch_igemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const 
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   at[0].val.programmaticStreamSerializationAllowed = 1;
   lc.attrs = at; lc.numAttrs = 1;
-  CZ_CUDA(cudaLaunchKernelEx(&lc, igemm::k_igemm<N_TILE>, tmA, tmB, tmOut, a));
+  CZ_CUDA(cudaLaunchKernelEx(&lc, igemm::k_igemm<N_TILE, M_TILE, CONV>, tmA, tmB, tmOut, a));
   CZ_CUDA(cudaGetLastError());
   return 0;
 }
@@ -149,11 +148,22 @@ int launch_igemm(int n_tile, const CUtensorMap& tmA, const CUtensorMap& tmB, con
   igemm::Args a = a0;
   a.staged = out_map && a.conv && !a.out_f32 && !a.residual && !a.residual32 && !a.out32;
   const CUtensorMap& tmOut = a.staged ? *out_map : tmA;    // not used unless staged
+  if (a.conv) {
+    const int key = n_tile * 1000 + a.tile_m;
+    switch (key) {                                          // the tiles conv_args chooses
+      case 64128: return launch_igemm_t<64, 128, true>(tmA, tmB, tmOut, a, st);
+      case 64256: return launch_igemm_t<64, 256, true>(tmA, tmB, tmOut, a, st);
+      case 128128: return launch_igemm_t<128, 128, true>(tmA, tmB, tmOut, a, st);
+      case 128256: return launch_igemm_t<128, 256, true>(tmA, tmB, tmOut, a, st);
+      case 192128: return launch_igemm_t<192, 128, true>(tmA, tmB, tmOut, a, st);
+    }
+    return cz_fail(CZ_ERR_UNSUPPORTED, "igemm: unsupported conv tile %d x %d", a.tile_m, n_tile);
+  }
   switch (n_tile) {
-    case 64: return launch_igemm_t<64>(tmA, tmB, tmOut, a, st);
-    case 128: return launch_igemm_t<128>(tmA, tmB, tmOut, a, st);
-    case 192: return launch_igemm_t<192>(tmA, tmB, tmOut, a, st);
-    case 256: return launch_igemm_t<256>(tmA, tmB, tmOut, a, st);
+    case 64: return launch_igemm_t<64, igemm::kTileM, false>(tmA, tmB, tmOut, a, st);
+    case 128: return launch_igemm_t<128, igemm::kTileM, false>(tmA, tmB, tmOut, a, st);
+    case 192: return launch_igemm_t<192, igemm::kTileM, false>(tmA, tmB, tmOut, a, st);
+    case 256: return launch_igemm_t<256, igemm::kTileM, false>(tmA, tmB, tmOut, a, st);
   }
   return cz_fail(CZ_ERR_UNSUPPORTED, "igemm: unsupported N tile %d (filters must be 64/128/192/256)", n_tile);
 }
@@ -164,11 +174,24 @@ static bool use_n_split(int n_boards, int c) {
   const int m_tiles = (n_boards * 90 + igemm::kTileM - 1) / igemm::kTileM;
   return m_tiles * (c / 64) <= num_sms();
 }
-igemm::Args conv_args(int n_boards, int c, const float* bias, const __half* residual, void* out, int relu) {
+// Conv tiles: N = 128 at C = 256 (two N tiles), C itself below; the small-batch form is 128 x 64.  M = 256 pixels (two m64
+// blocks per consumer warpgroup, 128 accumulators per thread at N = 128) halves the weight bytes each CTA loads per output
+// pixel, as long as the 256-pixel tiles fill at least 8 waves of CTAs: with fewer, the last, partly filled wave costs more
+// than the bytes save (c2, at most 2048 positions at 128x7, makes 720 such tiles, 5.5 waves, and ran 2.5 % slower with them on
+// an H100).  C = 192 stays
+// at 128 pixels: 2 x m64n192 would need 192 accumulators.
+int conv_tile_n(int c, bool split) { return split ? 64 : c == 256 ? 128 : c; }
+static int conv_tile_m(int n_boards, int c, bool split) {
+  if (split || c == 192) return 128;
+  const long long tiles = ((long long)n_boards * 90 + 255) / 256 * (c / conv_tile_n(c, false));
+  return tiles >= 8LL * num_sms() ? 256 : 128;
+}
+igemm::Args conv_args(int n_boards, int c, const float* bias, const __half* residual, void* out, int relu, bool split) {
   igemm::Args a;
   memset(&a, 0, sizeof(a));
   a.n_taps = 9; a.k_chunks = c / 64;
-  a.rows = n_boards * 90; a.m_tiles = (a.rows + 127) / 128; a.n_tiles = 1;
+  a.tile_m = conv_tile_m(n_boards, c, split);
+  a.rows = n_boards * 90; a.m_tiles = (a.rows + a.tile_m - 1) / a.tile_m; a.n_tiles = c / conv_tile_n(c, split);
   a.n_total = c; a.n_valid = c; a.ldo = c; a.conv = 1; a.relu = relu; a.out_f32 = 0;
   a.bias = bias; a.residual = residual; a.out = out; a.rows_per_unit = 90;
   return a;
@@ -178,7 +201,7 @@ static igemm::Args dense_args(int m, int n_valid, int n_pad, int k_pad, int n_ti
   igemm::Args a;
   memset(&a, 0, sizeof(a));
   a.n_taps = 1; a.k_chunks = k_pad / 64;
-  a.rows = m; a.m_tiles = (m + 127) / 128; a.n_tiles = n_pad / n_tile;
+  a.tile_m = igemm::kTileM; a.rows = m; a.m_tiles = (m + igemm::kTileM - 1) / igemm::kTileM; a.n_tiles = n_pad / n_tile;
   a.n_total = n_pad; a.n_valid = n_valid; a.ldo = ldo; a.conv = 0; a.relu = 0; a.out_f32 = 1;
   a.bias = bias; a.residual = nullptr; a.out = out;
   return a;
@@ -479,7 +502,7 @@ struct NetWeights {
   float *wh, *shifth, *wv1, *bv1, *wv2, *bv2;
   __half* w_pol; float* b_pol;
   CUtensorMap map_wpol;
-  std::vector<CUtensorMap> map_w;
+  std::vector<CUtensorMap> map_w;          // box rows = conv_tile_n(C, false)
   std::vector<CUtensorMap> map_w_64;       // box rows = 64: 64-column tiles of the small-batch launches (use_n_split)
   bool ready;                              // weights set (nn_set_weights)
 };
@@ -504,7 +527,7 @@ struct NnRuntime {
   float* scratch;                            // 2*C floats for BN folding
   CUtensorMap map_pf;                    // policy GEMM operand (pol_feat)
   bool fp32_skip;                        // keep the residual (skip) stream in fp32: halves the value error of deep nets, ~+30 % time
-  CUtensorMap imap_x, imap_t, imap_y;    // im2col maps of the three activation buffers
+  CUtensorMap hmap_x, hmap_t, hmap_y;    // the three activation buffers as the conv's halo loads read them
   CUtensorMap emap_t;                    // conv1's output buffer as the staged conv epilogue stores it
   // optional CUDA-event timing of the residual-tower launches (bench.py roofline)
   bool profile;
@@ -593,9 +616,9 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
   layout(r, cv);
   const int c = filters;
   int rc = 0;
-  rc |= make_map_im2col(&r->imap_x, r->x, c, max_batch);
-  rc |= make_map_im2col(&r->imap_t, r->t, c, max_batch);
-  rc |= make_map_im2col(&r->imap_y, r->y, c, max_batch);
+  rc |= make_map_2d(&r->hmap_x, r->x, c, (long long)max_batch * 90, igemm::kHaloBox);
+  rc |= make_map_2d(&r->hmap_t, r->t, c, (long long)max_batch * 90, igemm::kHaloBox);
+  rc |= make_map_2d(&r->hmap_y, r->y, c, (long long)max_batch * 90, igemm::kHaloBox);
   rc |= make_map_epi(&r->emap_t, r->t, c, (long long)max_batch * 90);
   rc |= make_map_2d(&r->map_pf, r->pol_feat, 3 * r->pol_k1, (long long)max_batch + 128, 128);
   for (int k = 0; k < n_nets; ++k) {
@@ -605,7 +628,7 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
     w.map_w.resize(2 * blocks);
     w.map_w_64.resize(2 * blocks);
     for (int i = 0; i < 2 * blocks; ++i) {
-      rc |= make_map_2d(&w.map_w[i], w.w_conv + (size_t)i * 9 * c * c, c, 9LL * c, c);
+      rc |= make_map_2d(&w.map_w[i], w.w_conv + (size_t)i * 9 * c * c, c, 9LL * c, conv_tile_n(c, false));
       rc |= make_map_2d(&w.map_w_64[i], w.w_conv + (size_t)i * 9 * c * c, c, 9LL * c, 64);
     }
   }
@@ -769,20 +792,19 @@ static int fw_tower(NnRuntime* r, const NetWeights& w, int n, const int* n_dev) 
   const int c = r->filters;
   cudaStream_t st = r->stream;
   float *x32 = r->fp32_skip ? r->x32 : nullptr, *y32 = r->fp32_skip ? r->y32 : nullptr;
-  CUtensorMap *ix = &r->imap_x, *iy = &r->imap_y;
+  CUtensorMap *ix = &r->hmap_x, *iy = &r->hmap_y;
   __half *x = r->x, *y = r->y;
   const bool split = use_n_split(n, c);
-  const int nt = split ? 64 : c;
+  const int nt = conv_tile_n(c, split);
   const std::vector<CUtensorMap>& wm = split ? w.map_w_64 : w.map_w;
   for (int i = 0; i < r->blocks; ++i) {
     // conv1: x -> t (no skip);  conv2: t (+ skip x or x32) -> y (+ y32)
-    igemm::Args d1 = conv_args(n, c, w.shift_conv + (size_t)(2 * i) * c, nullptr, r->t, 1);
-    igemm::Args d2 = conv_args(n, c, w.shift_conv + (size_t)(2 * i + 1) * c, x, y, 1);
+    igemm::Args d1 = conv_args(n, c, w.shift_conv + (size_t)(2 * i) * c, nullptr, r->t, 1, split);
+    igemm::Args d2 = conv_args(n, c, w.shift_conv + (size_t)(2 * i + 1) * c, x, y, 1, split);
     d1.n_dev = d2.n_dev = n_dev;
     d2.residual32 = x32; d2.out32 = y32;
-    d1.n_tiles = d2.n_tiles = c / nt;
     if (launch_igemm(nt, *ix, wm[2 * i], d1, st, &r->emap_t)) return CZ_ERR_CUDA;
-    if (launch_igemm(nt, r->imap_t, wm[2 * i + 1], d2, st)) return CZ_ERR_CUDA;
+    if (launch_igemm(nt, r->hmap_t, wm[2 * i + 1], d2, st)) return CZ_ERR_CUDA;
     r->launches += 2;
     std::swap(x, y); std::swap(x32, y32); std::swap(ix, iy);
   }
@@ -939,7 +961,7 @@ double nn_tower_flops_per_position(const NnRuntime* r) { return r ? 2.0 * 90.0 *
 // Building blocks exported for parity tests and profiling (not part of the reference-facing surface).
 extern "C" {
 
-// 3x3 "same" convolution on activations fp16 [n_boards][10][9][c] through the im2col TMA path:
+// 3x3 "same" convolution on activations fp16 [n_boards][10][9][c], the tower's full-width conv tiles:
 // out = relu?(conv(in, w) + bias (+ residual)); residual and out have the layout of in; w: fp16 [9][c_out = c][c_in = c],
 // bias f32 [c].
 int cz_igemm_conv3x3_dense(const void* act_in, const void* w, const float* bias, const void* residual, void* act_out,
@@ -947,10 +969,10 @@ int cz_igemm_conv3x3_dense(const void* act_in, const void* w, const float* bias,
   using namespace cznn;
   if (c % 64 || c < 64 || c > 256 || n_boards <= 0) return cz_fail(CZ_ERR_ARG, "cz_igemm_conv3x3_dense: bad shape");
   CUtensorMap ma, mb;
-  if (make_map_im2col(&ma, act_in, c, n_boards)) return CZ_ERR_CUDA;
-  if (make_map_2d(&mb, w, c, 9LL * c, c)) return CZ_ERR_CUDA;
+  if (make_map_2d(&ma, act_in, c, (long long)n_boards * 90, igemm::kHaloBox)) return CZ_ERR_CUDA;
+  if (make_map_2d(&mb, w, c, 9LL * c, conv_tile_n(c, false))) return CZ_ERR_CUDA;
   igemm::Args a = conv_args(n_boards, c, bias, (const __half*)residual, act_out, relu);
-  return launch_igemm(c, ma, mb, a, (cudaStream_t)stream);
+  return launch_igemm(conv_tile_n(c, false), ma, mb, a, (cudaStream_t)stream);
 }
 
 // out[m][n] = sum_k a[m][k] * w[n][k] + bias[n]; a fp16 [m_alloc >= ceil128(m)][k], w fp16 [n_pad][k], k % 64 == 0,

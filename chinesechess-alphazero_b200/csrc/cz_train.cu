@@ -485,8 +485,8 @@ struct Trainer {
   float *G, *D; __half* dz16;
   std::vector<__half*> wf16, wd16;   // [2L] forward / dgrad operands
   std::vector<CUtensorMap> map_wf, map_wd;
-  std::vector<CUtensorMap> im_a, im_h, im_a64, im_h64;
-  CUtensorMap im_dz, map_dz;
+  std::vector<CUtensorMap> hm_a, hm_h, im_a64, im_h64;   // conv inputs: halo maps (forward convs), im2col maps (wgrad)
+  CUtensorMap hm_dz, map_dz;
   float* wg_part; float* fw_part; float* col_part; float* gemm_part;
   float* scale_slots;                // [2L + 1][4]
   float *Fp, *Fv, *logits, *dlog, *hpre, *hact, *vpre, *dvpre, *dh, *dF, *ce_rows, *se_rows, *ones;
@@ -666,10 +666,11 @@ static int bn_backward(Trainer* t, Bn& b, long long P, const float* skip, const 
   return 0;
 }
 
-static igemm::Args conv_args(int n, int c, float* out) {
+// raw fp32 3x3 conv of fp16 activations (halo map `in`) with fp16 weights (map boxes of conv_tile_n rows)
+static int conv3x3(int n, int c, const CUtensorMap& in, const CUtensorMap& w, float* out, cudaStream_t st) {
   igemm::Args a = cznn::conv_args(n, c, nullptr, nullptr, out, 0);
   a.out_f32 = 1;
-  return a;
+  return cznn::launch_igemm(cznn::conv_tile_n(c, false), in, w, a, st);
 }
 
 template <int NB>
@@ -708,16 +709,17 @@ static int wgrad_launch(int c, int n, const CUtensorMap& dy, const CUtensorMap& 
 static int build_maps(Trainer* t, int n) {
   if (t->last_batch == n) return 0;
   const int C = t->C, L = t->L;
-  t->im_a.resize(L + 1); t->im_a64.resize(L + 1); t->im_h.resize(L); t->im_h64.resize(L);
+  const long long P = (long long)n * 90;
+  t->hm_a.resize(L + 1); t->im_a64.resize(L + 1); t->hm_h.resize(L); t->im_h64.resize(L);
   for (int k = 0; k <= L; ++k) {
-    CZ_TRY(cznn::make_map_im2col(&t->im_a[k], t->a16[k], C, n, 128));
+    CZ_TRY(cznn::make_map_2d(&t->hm_a[k], t->a16[k], C, P, igemm::kHaloBox));
     CZ_TRY(cznn::make_map_im2col(&t->im_a64[k], t->a16[k], C, n, wgrad::kPix));
   }
   for (int k = 0; k < L; ++k) {
-    CZ_TRY(cznn::make_map_im2col(&t->im_h[k], t->h16[k], C, n, 128));
+    CZ_TRY(cznn::make_map_2d(&t->hm_h[k], t->h16[k], C, P, igemm::kHaloBox));
     CZ_TRY(cznn::make_map_im2col(&t->im_h64[k], t->h16[k], C, n, wgrad::kPix));
   }
-  CZ_TRY(cznn::make_map_im2col(&t->im_dz, t->dz16, C, n, 128));
+  CZ_TRY(cznn::make_map_2d(&t->hm_dz, t->dz16, C, P, igemm::kHaloBox));
   CZ_TRY(cznn::make_map_2d(&t->map_dz, t->dz16, C, (long long)n * 90, wgrad::kPix));
   t->last_batch = n;
   return 0;
@@ -738,9 +740,9 @@ static int step(Trainer* t, const float* planes, const float* pol_t, const float
   CZ_TRY(bn_forward(t, t->bn[0], P, nullptr, t->a16[0], t->s32[0], 0));
   for (int i = 0; i < L; ++i) {
     Bn &b1 = t->bn[1 + 2 * i], &b2 = t->bn[2 + 2 * i];
-    CZ_TRY(cznn::launch_igemm(C, t->im_a[i], t->map_wf[2 * i], conv_args(n, C, b1.z), st));
+    CZ_TRY(conv3x3(n, C, t->hm_a[i], t->map_wf[2 * i], b1.z, st));
     CZ_TRY(bn_forward(t, b1, P, nullptr, t->h16[i], nullptr, 0));
-    CZ_TRY(cznn::launch_igemm(C, t->im_h[i], t->map_wf[2 * i + 1], conv_args(n, C, b2.z), st));
+    CZ_TRY(conv3x3(n, C, t->hm_h[i], t->map_wf[2 * i + 1], b2.z, st));
     CZ_TRY(bn_forward(t, b2, P, t->s32[i], t->a16[i + 1], t->s32[i + 1], 0));
   }
   const float* S = t->s32[L];
@@ -785,13 +787,13 @@ static int step(Trainer* t, const float* planes, const float* pol_t, const float
     k_pick_scale<<<1, 1, 0, st>>>(slot2);
     k_to_half_scaled<<<blocks_for(PC), 256, 0, st>>>(c2.z, PC, slot2, t->dz16);
     CZ_TRY(wgrad_launch(C, n, t->map_dz, t->im_h64[i], t->wg_part, slot2, t->p[t->i_conv[2 * i + 1]].g, st));
-    CZ_TRY(cznn::launch_igemm(C, t->im_dz, t->map_wd[2 * i + 1], conv_args(n, C, t->D), st));
+    CZ_TRY(conv3x3(n, C, t->hm_dz, t->map_wd[2 * i + 1], t->D, st));
     // conv1: D * inv2 (gradient of the conv1 activation) -> dz1
     CZ_TRY(bn_backward(t, c1, P, nullptr, t->D, slot2 + 2, 0, nullptr, slot1));
     k_pick_scale<<<1, 1, 0, st>>>(slot1);
     k_to_half_scaled<<<blocks_for(PC), 256, 0, st>>>(c1.z, PC, slot1, t->dz16);
     CZ_TRY(wgrad_launch(C, n, t->map_dz, t->im_a64[i], t->wg_part, slot1, t->p[t->i_conv[2 * i]].g, st));
-    CZ_TRY(cznn::launch_igemm(C, t->im_dz, t->map_wd[2 * i], conv_args(n, C, t->D), st));
+    CZ_TRY(conv3x3(n, C, t->hm_dz, t->map_wd[2 * i], t->D, st));
     k_add_scaled<<<blocks_for(PC), 256, 0, st>>>(t->G, t->D, PC, slot1 + 2);
   }
   CZ_TRY(bn_backward(t, t->bn[0], P, nullptr, t->G, nullptr, 0, nullptr, nullptr));
@@ -866,8 +868,8 @@ int cz_train_create(const cz_train_config* cfg, void* workspace, uint64_t bytes,
   t->map_wf.resize(2 * t->L); t->map_wd.resize(2 * t->L);
   int rc = 0;
   for (int l = 0; l < 2 * t->L && !rc; ++l) {
-    rc |= cznn::make_map_2d(&t->map_wf[l], t->wf16[l], C, 9LL * C, C);
-    rc |= cznn::make_map_2d(&t->map_wd[l], t->wd16[l], C, 9LL * C, C);
+    rc |= cznn::make_map_2d(&t->map_wf[l], t->wf16[l], C, 9LL * C, cznn::conv_tile_n(C, false));
+    rc |= cznn::make_map_2d(&t->map_wd[l], t->wd16[l], C, 9LL * C, cznn::conv_tile_n(C, false));
   }
   if (rc) { delete h; return CZ_ERR_CUDA; }
   k_fill<<<blocks_for(t->maxb), 256, 0, t->st>>>(t->ones, t->maxb, 1.f);
@@ -1058,15 +1060,15 @@ int cz_train_dgrad3x3(const float* dy, const float* w_hwio, int n, int c, float*
   CZ_CUDA(cudaMalloc(&wd, 9ULL * c * c * 2));
   CZ_CUDA(cudaMalloc(&slot, 16));
   CUtensorMap ma, mb;
-  int rc = cznn::make_map_im2col(&ma, d16, c, n, 128);
-  if (!rc) rc = cznn::make_map_2d(&mb, wd, c, 9LL * c, c);
+  int rc = cznn::make_map_2d(&ma, d16, c, P, igemm::kHaloBox);
+  if (!rc) rc = cznn::make_map_2d(&mb, wd, c, 9LL * c, cznn::conv_tile_n(c, false));
   if (!rc) {
     cudaMemsetAsync(slot, 0, 16, st);
     k_prep_conv3_train<<<blocks_for(9LL * c * c), 256, 0, st>>>(w_hwio, wf, wd, c);
     k_absmax<<<blocks_for(P * c), 256, 0, st>>>(dy, P * c, reinterpret_cast<unsigned*>(slot));
     k_pick_scale<<<1, 1, 0, st>>>(slot);
     k_to_half_scaled<<<blocks_for(P * c), 256, 0, st>>>(dy, P * c, slot, d16);
-    rc = cznn::launch_igemm(c, ma, mb, conv_args(n, c, dx), st);
+    rc = conv3x3(n, c, ma, mb, dx, st);
     if (!rc) k_scale<<<blocks_for(P * c), 256, 0, st>>>(dx, P * c, slot + 2);
   }
   cudaStreamSynchronize(st);
