@@ -443,6 +443,20 @@ __global__ void __launch_bounds__(128) k_legal_priors(const float* __restrict__ 
 }
 __global__ void k_set_int(int* p, int v) { *p = v; }
 
+// Profiling bracket around the residual tower (nn_profile): one thread each, ordered by the stream.  Kernel nodes rather
+// than event records, so that a WHILE node's body graph can hold them.  prof = {start, ns, brackets, positions}.
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__global__ void k_prof_begin(unsigned long long* prof) { prof[0] = global_ns(); }
+__global__ void k_prof_end(unsigned long long* prof, const int* __restrict__ n_dev) {
+  prof[1] += global_ns() - prof[0];
+  prof[2] += 1;
+  prof[3] += (unsigned long long)*n_dev;
+}
+
 // ---- weight preparation (Keras layout f32 -> folded operands)
 __global__ void k_bn_fold(const float* gamma, const float* beta, const float* mean, const float* var, float* scale,
                           float* shift, int c) {
@@ -520,8 +534,6 @@ struct NnRuntime {
   float2* stats;                         // [max_batch][kPolN / 256] softmax statistics of the policy GEMM's N tiles
   int* n_scalar;                         // device copy of a host-known batch size (reference-facing forward)
   bool heads_attr;                       // k_heads was granted > 48 KB of dynamic shared memory (wide legacy heads)
-  bool capturing;                        // inside cudaStreamBeginCapture: no event records / synchronisation
-  size_t prof_open;                      // event pair opened by nn_prof_begin
   uint8_t* boards_tmp;
   int in_planes;                         // 14, or 28 with use_history (board + history board per position)
   float* scratch;                            // 2*C floats for BN folding
@@ -529,23 +541,11 @@ struct NnRuntime {
   bool fp32_skip;                        // keep the residual (skip) stream in fp32: halves the value error of deep nets, ~+30 % time
   CUtensorMap hmap_x, hmap_t, hmap_y;    // the three activation buffers as the conv's halo loads read them
   CUtensorMap emap_t;                    // conv1's output buffer as the staged conv epilogue stores it
-  // optional CUDA-event timing of the residual-tower launches (bench.py roofline)
+  // optional timing of the residual tower (bench.py roofline): with `profile` on, every forward brackets its tower with
+  // k_prof_begin / k_prof_end, which accumulate into prof[4] = {start, ns, brackets, positions}
   bool profile;
-  std::vector<cudaEvent_t> ev;        // pairs, recycled
-  size_t ev_used;
-  std::vector<double> ev_flops;       // algorithmic flops bracketed by pair i
-  double prof_ms, prof_flops; uint64_t prof_launches;
+  unsigned long long* prof;
 };
-
-static void prof_collect(NnRuntime* r) {
-  for (size_t i = 0; i + 1 < r->ev_used; i += 2) {
-    float ms = 0.f;
-    if (cudaEventElapsedTime(&ms, r->ev[i], r->ev[i + 1]) == cudaSuccess) {
-      r->prof_ms += ms; r->prof_flops += r->ev_flops[i / 2]; r->prof_launches += (uint64_t)(2 * r->blocks);
-    }
-  }
-  r->ev_used = 0;
-}
 
 static void layout(NnRuntime* r, Carver& cv) {
   const int c = r->filters;
@@ -560,6 +560,7 @@ static void layout(NnRuntime* r, Carver& cv) {
   r->stats = (float2*)cv.take((size_t)r->max_batch * (kPolN / 256) * sizeof(float2));
   r->n_scalar = (int*)cv.take(64);
   r->boards_tmp = (uint8_t*)cv.take((size_t)r->max_batch * 2 * CZ_BOARD_STRIDE);
+  r->prof = (unsigned long long*)cv.take(4 * sizeof(unsigned long long));
   for (int k = 0; k < r->n_nets; ++k) {
     NetWeights& w = r->nets[k];
     w.w_first = (__half*)cv.take((size_t)25 * 28 * c * sizeof(__half));
@@ -611,7 +612,7 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
   // past 1e-3: value 1.1e-3 .. 1.5e-3 at 20 random-init blocks vs <= 6e-4 with fp32; policy 1.6e-3 vs 9.8e-4 on the
   // reference's trained 192x10 net), 1 = always, 2 = never
   r->fp32_skip = fp32_skip_mode == 1 || (fp32_skip_mode == 0 && blocks >= 10);
-  r->profile = false; r->ev_used = 0; r->prof_ms = 0; r->prof_flops = 0; r->prof_launches = 0; r->capturing = false;
+  r->profile = false;
   Carver cv{(uint8_t*)workspace, 0};
   layout(r, cv);
   const int c = filters;
@@ -639,24 +640,23 @@ NnRuntime* nn_create(int device, int filters, int blocks, int value_fc, int max_
   cudaMemsetAsync(r->t, 0, (size_t)max_batch * 90 * c * 2, r->stream);
   cudaMemsetAsync(r->y, 0, (size_t)max_batch * 90 * c * 2, r->stream);
   cudaMemsetAsync(r->pol_feat, 0, ((size_t)max_batch + 128) * 3 * r->pol_k1 * 2, r->stream);
+  cudaMemsetAsync(r->prof, 0, 4 * sizeof(unsigned long long), r->stream);
   return r;
 }
 
-void nn_destroy(NnRuntime* r) {
-  if (!r) return;
-  for (cudaEvent_t e : r->ev) cudaEventDestroy(e);
-  delete r;
-}
+void nn_destroy(NnRuntime* r) { delete r; }
 void nn_profile(NnRuntime* r, bool on) { if (r) { r->profile = on; } }
-// Synchronises the stream. ms = device time spent in the residual-tower igemm launches since the last read.
+// Synchronises the stream.  ms = device time spent in the residual towers bracketed since the last read, launches = their
+// igemm launches, flops = their algorithmic flops (2*90*9*C*C per position per conv); clears the accumulators.
 int nn_profile_read(NnRuntime* r, double* ms, uint64_t* launches, double* flops) {
   if (!r) return cz_fail(CZ_ERR_STATE, "no network");
+  unsigned long long p[4];
+  CZ_CUDA(cudaMemcpyAsync(p, r->prof, sizeof(p), cudaMemcpyDeviceToHost, r->stream));
+  CZ_CUDA(cudaMemsetAsync(r->prof, 0, sizeof(p), r->stream));
   CZ_CUDA(cudaStreamSynchronize(r->stream));
-  prof_collect(r);
-  if (ms) *ms = r->prof_ms;
-  if (launches) *launches = r->prof_launches;
-  if (flops) *flops = r->prof_flops;
-  r->prof_ms = 0; r->prof_flops = 0; r->prof_launches = 0;
+  if (ms) *ms = (double)p[1] * 1e-6;
+  if (launches) *launches = p[2] * (uint64_t)(2 * r->blocks);
+  if (flops) *flops = (double)p[3] * (2.0 * 90.0 * 9.0 * r->filters * r->filters * 2.0 * r->blocks);
   return 0;
 }
 bool nn_ready(const NnRuntime* r) {
@@ -769,7 +769,6 @@ int nn_set_weights(NnRuntime* r, int net, const cz_tensor_desc* descs, int n_des
 // One pass over at most `n_max` positions; the ACTUAL batch size is the device integer *n_dev (every launch has a fixed
 // shape sized for n_max, kernels read *n_dev and leave the rest untouched), so a search never has to tell the host how
 // many leaves a wave produced.  Leaves logits [n][kPolN] + per-tile softmax statistics in r->logits / r->stats.
-// The three parts are separate so that the search can capture them into three CUDA graphs and bracket the tower with events.
 static int conv_first_threads(int c) {                    // (c/2) channel pairs x as many pixel groups as fit 256 threads
   const int pairs = c / 2;
   int g = 256 / pairs;
@@ -831,29 +830,17 @@ static int fw_heads(NnRuntime* r, const NetWeights& w, int n, const int* n_dev, 
   CZ_CUDA(cudaGetLastError());
   return 0;
 }
-// events around the tower of one forward (bench.py roofline); flops = algorithmic flops of the bracketed launches, or < 0 when
-// only the device knows the batch size (the reader then takes the positions from the search's device counter)
-void nn_prof_begin(NnRuntime* r, double flops) {
-  r->prof_open = (size_t)-1;
-  if (!r->profile) return;
-  if (r->ev_used + 2 > 4096) { cudaStreamSynchronize(r->stream); prof_collect(r); }
-  while (r->ev.size() < r->ev_used + 2) { cudaEvent_t e; cudaEventCreate(&e); r->ev.push_back(e); }
-  r->prof_open = r->ev_used; r->ev_used += 2;
-  if (r->ev_flops.size() < r->ev_used / 2) r->ev_flops.resize(r->ev_used / 2);
-  r->ev_flops[r->prof_open / 2] = flops > 0 ? flops : 0.0;
-  cudaEventRecord(r->ev[r->prof_open], r->stream);
-}
-void nn_prof_end(NnRuntime* r) {
-  if (r->prof_open != (size_t)-1) cudaEventRecord(r->ev[r->prof_open + 1], r->stream);
-  r->prof_open = (size_t)-1;
-}
+// first conv, residual tower (bracketed by k_prof_begin / k_prof_end while profiling is on), heads + policy GEMM
 static int forward_tower(NnRuntime* r, const NetWeights& w, const uint8_t* boards, int n_max, const int* n_dev, float* value) {
   int rc = fw_first(r, w, boards, n_max, n_dev);
   if (rc) return rc;
-  nn_prof_begin(r, 2.0 * 90.0 * 9.0 * r->filters * r->filters * (double)n_max * 2.0 * r->blocks);
+  if (r->profile) k_prof_begin<<<1, 1, 0, r->stream>>>(r->prof);
   rc = fw_tower(r, w, n_max, n_dev);
-  nn_prof_end(r);
   if (rc) return rc;
+  if (r->profile) {
+    k_prof_end<<<1, 1, 0, r->stream>>>(r->prof, n_dev);
+    r->launches += 2;
+  }
   return fw_heads(r, w, n_max, n_dev, value);
 }
 
@@ -894,22 +881,18 @@ int nn_forward_planes(NnRuntime* r, int net, const float* planes, int batch, flo
 
 // The search's evaluation step: up to n_max leaves (actual count *n_dev), boards + legal-move labels in, value [n] and the
 // softmax probabilities of the legal moves [n][CZ_MAX_MOVES] out.  Fixed launch shapes: safe to capture into a CUDA graph.
-int nn_forward_leaves(NnRuntime* r, int net, int part, const uint8_t* boards, int n_max, const int* n_dev, const int16_t* labels,
+int nn_forward_leaves(NnRuntime* r, int net, const uint8_t* boards, int n_max, const int* n_dev, const int16_t* labels,
                       const int32_t* label_counts, float* legal_p, float* value) {
   const NetWeights* w = ready_net(r, net);
   if (!w) return CZ_ERR_STATE;
   if (n_max > r->max_batch) return cz_fail(CZ_ERR_ARG, "nn_forward_leaves: %d leaves > max batch %d", n_max, r->max_batch);
-  int rc = 0;
-  if (part & 1) rc = fw_first(r, *w, boards, n_max, n_dev);
-  if (!rc && (part & 2)) rc = fw_tower(r, *w, n_max, n_dev);
-  if (!rc && (part & 4)) rc = fw_heads(r, *w, n_max, n_dev, value);
+  const int rc = forward_tower(r, *w, boards, n_max, n_dev, value);
   if (rc) return rc;
-  if (part & 4) k_legal_priors<<<(n_max + 3) / 4, 128, 0, r->stream>>>(r->logits, kPolN, r->stats, kPolN / 256, labels, label_counts, n_dev, legal_p);
-  if (part & 4) r->launches++;
+  k_legal_priors<<<(n_max + 3) / 4, 128, 0, r->stream>>>(r->logits, kPolN, r->stats, kPolN / 256, labels, label_counts, n_dev, legal_p);
+  r->launches++;
   CZ_CUDA(cudaGetLastError());
   return 0;
 }
-void nn_set_capturing(NnRuntime* r, bool on) { if (r) r->capturing = on; }
 bool nn_profiling(const NnRuntime* r) { return r && r->profile; }
 // Parity tests: copy rows of an intermediate buffer out after a forward.  Which physical buffer holds a stage follows the
 // ping-pong of fw_tower and the choice fw_heads makes (x <-> y once per block, the fp32 copies alongside).  Off the forward
@@ -952,8 +935,7 @@ int nn_read_buffer(NnRuntime* r, int which, int n, void* dst, long long dst_byte
   CZ_CUDA(cudaStreamSynchronize(r->stream));
   return 0;
 }
-int nn_launches_per_forward(const NnRuntime* r) { return r ? 1 + 2 * r->blocks + 3 : 0; }
-double nn_tower_flops_per_position(const NnRuntime* r) { return r ? 2.0 * 90.0 * 9.0 * r->filters * r->filters * 2.0 * r->blocks : 0.0; }
+int nn_launches_per_forward(const NnRuntime* r) { return r ? 1 + 2 * r->blocks + 3 + (r->profile ? 2 : 0) : 0; }
 
 }  // namespace cznn
 

@@ -24,17 +24,13 @@ int nn_forward_planes(NnRuntime*, int net, const float* planes_dev, int batch, f
 // shapes, capturable into a CUDA graph).  labels_dev [n][CZ_MAX_MOVES] int16 = action label of every legal move (-1: none),
 // label_counts_dev [n]; legal_p_dev [n][CZ_MAX_MOVES] f32 gets the softmax probability of exactly those labels — bit for bit
 // the numbers nn_forward_boards writes at those indices of its [n][2086] vector.
-// part: bit 0 = first convolution, bit 1 = residual tower (the tensor-core launches), bit 2 = heads + policy GEMM + legal priors;
-// 7 = everything.  The parts of one evaluation must run in this order on the runtime's stream.
-int nn_forward_leaves(NnRuntime*, int net, int part, const uint8_t* boards_dev, int n_max, const int* n_dev, const int16_t* labels_dev,
+int nn_forward_leaves(NnRuntime*, int net, const uint8_t* boards_dev, int n_max, const int* n_dev, const int16_t* labels_dev,
                       const int32_t* label_counts_dev, float* legal_p_dev, float* value_dev);
-void nn_set_capturing(NnRuntime*, bool on);
 bool nn_profiling(const NnRuntime*);
-void nn_prof_begin(NnRuntime*, double flops);   // event bracket around the tower launches when profiling is on (not capturable)
-void nn_prof_end(NnRuntime*);
+// launches of one nn_forward_leaves, the two profiling stamps included while profiling is on
 int nn_launches_per_forward(const NnRuntime*);
-double nn_tower_flops_per_position(const NnRuntime*);
 uint64_t nn_launches(const NnRuntime*);
+// While on, every forward brackets its residual tower with two stamp kernels (capturable, like the rest of the forward).
 void nn_profile(NnRuntime*, bool on);
 int nn_profile_read(NnRuntime*, double* ms, uint64_t* launches, double* flops);
 // cz_nn_read_buffer (include/cczero_b200.h): rows of an intermediate buffer of the last forward; synchronises

@@ -136,24 +136,16 @@ CZ_KERNEL(k_gather)(EngineDev E, int g0, int g1, uint8_t* dense, int16_t* labels
     if (czs::lane() == 0) nlab[off + j] = L;
   }
 }
-// Device-driven search loop: after every iteration tell the polling host thread (mapped pinned memory) how many iterations
-// are complete and whether any range still has work.  flags[1] (busy) is written before flags[0] (count).
-CZ_KERNEL(k_loop_flag)(EngineDev E, int n_slots, volatile int32_t* flags, unsigned long long cond_handle, int set_cond) {
+// Device-driven search loop, end of an iteration: count it in *iters (mapped pinned memory, read by the host after the
+// search's synchronise for cz_launch_count) and, inside the WHILE node's body, run the body again while any range has work.
+CZ_KERNEL(k_loop_flag)(EngineDev E, int n_slots, int32_t* iters, unsigned long long cond_handle, int set_cond) {
   if (czs::lane() != 0) return;
   int busy = 0;
   for (int s = 0; s < n_slots; ++s) busy |= (E.totals[4 * s] > 0) | (E.totals[4 * s + 1] != 0);
   const int it = E.loop_iter[0] + 1;
   E.loop_iter[0] = it;
-  unsigned long long n_eval = 0;                         // positions the device-driven loop evaluated (cz_nn_profile's flops)
-  for (int s = 0; s < n_slots; ++s) n_eval += (unsigned long long)E.totals[4 * s];
-  E.counters[0] += n_eval;
-  flags[1] = busy;
+  *iters = it;
 #if !defined(CZ_EMUL)
-  __threadfence_system();
-#endif
-  flags[0] = it;
-#if !defined(CZ_EMUL)
-  // WHILE-node form of the loop (the whole search is ONE graph launch): the body runs again while any range has work
   if (set_cond) cudaGraphSetConditional((cudaGraphConditionalHandle)cond_handle, busy ? 1u : 0u);
 #else
   (void)cond_handle; (void)set_cond;
@@ -335,24 +327,19 @@ struct cz_engine {
   int32_t* stat_n; uint16_t* stat_mv; int32_t* stat_cnt;    // staging for cz_get_root_stats
   int32_t* sims_stage;                                      // [G] staging for cz_set_game_sims
   int last_leaves;
-  unsigned long long prof_pos0;                             // device counter [0] at the last cz_nn_profile read
-  bool own_stream;                                          // e->stream was created by cz_create (caller passed the default stream)
+  bool own_stream;                                         // e->stream was created by cz_create (caller passed the default stream)
   int ring_count;                                           // finished-game records in the device ring (as of the last cz_play_move)
   uint64_t launches;
   uint64_t total_sims;
 #if !defined(CZ_EMUL)
   cznn::NnRuntime* nn;
   size_t nn_bytes;
-  // device-driven search loop: one iteration = three captured graphs per game range (tree work + first conv | residual
-  // tower | heads + legal priors), launched back to back; the host only polls h_flags (mapped pinned memory)
-  cudaGraphExec_t g_pre[2], g_tower[2], g_post[2];
-  cudaGraphExec_t g_while;                                  // the whole loop as one graph: WHILE conditional node around the iteration
-  unsigned long long while_handle;
-  int capture_cond;                                         // 1 while capturing the body of g_while (k_loop_flag sets the condition)
+  // the device-driven search loop as one graph: a WHILE conditional node around the iteration; [0] the production form,
+  // [1] with the residual towers bracketed by the profiling stamps (captured at the first search with cz_nn_profile on)
+  cudaGraphExec_t g_while[2];
   int n_ranges;                                             // 1, or 2 in arena mode (one network per range)
-  bool graphs_built;
-  volatile int32_t* h_flags;                                // mapped pinned [4]: iterations finished, busy
-  int32_t* d_flags;                                         // device view of h_flags
+  volatile int32_t* h_iters;                                // mapped pinned: iterations of the last search loop (k_loop_flag)
+  int32_t* d_iters;                                         // device view of h_iters
 #endif
 };
 
@@ -490,7 +477,7 @@ int cz_create(const cz_config* cfg, void* workspace, uint64_t workspace_bytes, v
   if (!e) return cz_fail(CZ_ERR_STATE, "cz_create: out of host memory");
   e->cfg = *cfg;
   e->stream = (cz_stream_t)stream;
-  e->own_stream = false; e->prof_pos0 = 0;
+  e->own_stream = false;
   e->ws = (uint8_t*)workspace; e->ws_bytes = workspace_bytes;
   e->launches = 0; e->last_leaves = 0; e->ring_count = 0; e->total_sims = 0;
   EngineDev& d = e->d;
@@ -504,9 +491,8 @@ int cz_create(const cz_config* cfg, void* workspace, uint64_t workspace_bytes, v
   const size_t used = carve(e, e->ws);
 #if !defined(CZ_EMUL)
   e->nn = nullptr; e->nn_bytes = 0;
-  e->graphs_built = false; e->h_flags = nullptr; e->d_flags = nullptr; e->n_ranges = cfg->arena ? 2 : 1;
-  for (int i = 0; i < 2; ++i) { e->g_pre[i] = e->g_tower[i] = e->g_post[i] = nullptr; }
-  e->g_while = nullptr; e->while_handle = 0; e->capture_cond = 0;
+  e->h_iters = nullptr; e->d_iters = nullptr; e->n_ranges = cfg->arena ? 2 : 1;
+  e->g_while[0] = e->g_while[1] = nullptr;
   if (cudaSetDevice(cfg->device) != cudaSuccess) { delete e; return cz_fail(CZ_ERR_CUDA, "cz_create: cudaSetDevice(%d) failed", cfg->device); }
   if (!e->stream) {
     // The legacy default stream cannot be captured into a graph.  A BLOCKING stream of our own keeps the caller's ordering:
@@ -517,10 +503,10 @@ int cz_create(const cz_config* cfg, void* workspace, uint64_t workspace_bytes, v
   }
   if (cfg->nn_filters > 0) {
     void* hf = nullptr;
-    if (cudaHostAlloc(&hf, 64, cudaHostAllocMapped) != cudaSuccess || cudaHostGetDevicePointer((void**)&e->d_flags, hf, 0) != cudaSuccess) {
-      delete e; return cz_fail(CZ_ERR_CUDA, "cz_create: mapped host memory for the loop flags failed");
+    if (cudaHostAlloc(&hf, 64, cudaHostAllocMapped) != cudaSuccess || cudaHostGetDevicePointer((void**)&e->d_iters, hf, 0) != cudaSuccess) {
+      delete e; return cz_fail(CZ_ERR_CUDA, "cz_create: mapped host memory for the loop's iteration count failed");
     }
-    e->h_flags = (volatile int32_t*)hf;
+    e->h_iters = (volatile int32_t*)hf;
     memset(hf, 0, 64);
   }
 #endif
@@ -555,14 +541,10 @@ void cz_destroy(cz_engine* e) {
   if (!e) return;
 #if !defined(CZ_EMUL)
   cznn::nn_destroy(e->nn);
-  if (e->h_flags) cudaFreeHost((void*)e->h_flags);
+  if (e->h_iters) cudaFreeHost((void*)e->h_iters);
   if (e->own_stream) { cudaStreamSynchronize(e->stream); cudaStreamDestroy(e->stream); }
-  for (int i = 0; i < 2; ++i) {
-    if (e->g_pre[i]) cudaGraphExecDestroy(e->g_pre[i]);
-    if (e->g_tower[i]) cudaGraphExecDestroy(e->g_tower[i]);
-    if (e->g_post[i]) cudaGraphExecDestroy(e->g_post[i]);
-  }
-  if (e->g_while) cudaGraphExecDestroy(e->g_while);
+  for (int i = 0; i < 2; ++i)
+    if (e->g_while[i]) cudaGraphExecDestroy(e->g_while[i]);
 #endif
   delete e;
 }
@@ -728,8 +710,7 @@ namespace {
 // Range h = games [gb, ge) evaluated by network h (arena: player h's trees; otherwise one range = all games).  One iteration
 // of a range:   apply(previous evaluation) -> wave -> scan -> gather(+labels) -> first conv | tower | heads, policy GEMM,
 // legal priors.  Every launch has a fixed shape; the number of leaves is the device integer totals[4h] that k_scan writes and
-// every network kernel reads, so nothing has to come back to the host between waves.  The three parts are captured once as
-// CUDA graphs; the tower graph is separate only so that cz_nn_profile can bracket it with events.
+// every network kernel reads, so nothing has to come back to the host between waves.
 struct Range { int gb, ge; uint8_t* dense; int16_t* labels; int32_t* nlab; float* legal_p; float* value; };
 Range range_of(cz_engine* e, int h) {
   const int G = e->cfg.n_games, K = e->cfg.leaves_per_round;
@@ -742,25 +723,25 @@ Range range_of(cz_engine* e, int h) {
   r.legal_p = e->legal_p + off * MAX_MOVES; r.value = e->value_buf + off;
   return r;
 }
-// the launches of one part of one range's iteration (part 1: tree work + first conv, 2: tower, 4: heads + priors + loop flag)
-int enqueue_part(cz_engine* e, int h, int part) {
-  const Range r = range_of(e, h);
-  const int n_max = (r.ge - r.gb) * e->cfg.leaves_per_round;
-  const int* n_dev = e->d.totals + 4 * h;
-  if (part == 1) {
+// the launches of one iteration of every range, then k_loop_flag; `cond`: the handle of the WHILE node whose body is being
+// captured, null for plain launches
+int enqueue_iteration(cz_engine* e, const cudaGraphConditionalHandle* cond) {
+  for (int h = 0; h < e->n_ranges; ++h) {
+    const Range r = range_of(e, h);
+    const int n_max = (r.ge - r.gb) * e->cfg.leaves_per_round;
     RANGE_LAUNCH(e, e->stream, r.gb, r.ge, k_apply_wave, e->d, r.gb, r.ge, (const float*)r.legal_p, (const float*)r.value);
     k_scan_block<<<1, 1024, 0, e->stream>>>(e->d, r.gb, r.ge, h);
     RANGE_LAUNCH(e, e->stream, r.gb, r.ge, k_gather, e->d, r.gb, r.ge, r.dense, r.labels, r.nlab);
+    const int rc = cznn::nn_forward_leaves(e->nn, e->cfg.arena ? h : 0, r.dense, n_max, e->d.totals + 4 * h, r.labels, r.nlab, r.legal_p, r.value);
+    if (rc) return rc;
   }
-  const int rc = cznn::nn_forward_leaves(e->nn, e->cfg.arena ? h : 0, part, r.dense, n_max, n_dev, r.labels, r.nlab, r.legal_p, r.value);
-  if (rc) return rc;
-  if (part == 4 && h == e->n_ranges - 1)
-    CZ_LAUNCH(k_loop_flag, 1, 1, 0, e->stream, e->d, e->n_ranges, (volatile int32_t*)e->d_flags, e->while_handle, e->capture_cond);
+  CZ_LAUNCH(k_loop_flag, 1, 1, 0, e->stream, e->d, e->n_ranges, e->d_iters, cond ? (unsigned long long)*cond : 0ULL, cond ? 1 : 0);
   return 0;
 }
 // The whole loop as ONE graph: a WHILE conditional node whose body is one iteration of every range; k_loop_flag ends each
 // iteration by setting the condition to "some range still has work".  No host involvement until the final synchronise.
-int build_while_graph(cz_engine* e) {
+// Captured with profiling as it is now (nn_profile), into g_while[profiled].
+int build_while_graph(cz_engine* e, int profiled) {
   cudaGraph_t g = nullptr;
   if (cudaGraphCreate(&g, 0) != cudaSuccess) return cz_fail(CZ_ERR_CUDA, "cudaGraphCreate failed");
   cudaGraphConditionalHandle handle;
@@ -778,114 +759,40 @@ int build_while_graph(cz_engine* e) {
     return cz_fail(CZ_ERR_CUDA, "cudaGraphAddNode(conditional) failed: %s", cudaGetErrorString(cudaGetLastError()));
   }
   cudaGraph_t body = np.conditional.phGraph_out[0];
-  e->while_handle = (unsigned long long)handle;
-  e->capture_cond = 1;
-  cznn::nn_set_capturing(e->nn, true);
   int rc = 0;
   if (cudaStreamBeginCaptureToGraph(e->stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) != cudaSuccess) {
     rc = cz_fail(CZ_ERR_CUDA, "cudaStreamBeginCaptureToGraph failed: %s", cudaGetErrorString(cudaGetLastError()));
   } else {
-    for (int h = 0; h < e->n_ranges && !rc; ++h)
-      for (int part = 1; part <= 4 && !rc; part <<= 1) rc = enqueue_part(e, h, part);
+    rc = enqueue_iteration(e, &handle);
     cudaGraph_t out = nullptr;
     const cudaError_t err = cudaStreamEndCapture(e->stream, &out);
     if (!rc && err != cudaSuccess) rc = cz_fail(CZ_ERR_CUDA, "capture of the loop body failed: %s", cudaGetErrorString(err));
   }
-  cznn::nn_set_capturing(e->nn, false);
-  e->capture_cond = 0;
-  if (!rc && cudaGraphInstantiate(&e->g_while, g, 0) != cudaSuccess)
+  if (!rc && cudaGraphInstantiate(&e->g_while[profiled], g, 0) != cudaSuccess)
     rc = cz_fail(CZ_ERR_CUDA, "instantiate of the WHILE graph failed: %s", cudaGetErrorString(cudaGetLastError()));
   cudaGraphDestroy(g);
   return rc;
-}
-int capture_part(cz_engine* e, int h, int part, cudaGraphExec_t* out) {
-  cznn::nn_set_capturing(e->nn, true);
-  if (cudaStreamBeginCapture(e->stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) {
-    cznn::nn_set_capturing(e->nn, false);
-    return cz_fail(CZ_ERR_CUDA, "cudaStreamBeginCapture failed: %s", cudaGetErrorString(cudaGetLastError()));
-  }
-  const int rc = enqueue_part(e, h, part);
-  cudaGraph_t g = nullptr;
-  cudaError_t err = cudaStreamEndCapture(e->stream, &g);
-  cznn::nn_set_capturing(e->nn, false);
-  if (rc) { if (g) cudaGraphDestroy(g); return rc; }
-  if (err != cudaSuccess || !g) return cz_fail(CZ_ERR_CUDA, "graph capture (range %d part %d) failed: %s", h, part, cudaGetErrorString(err));
-  err = cudaGraphInstantiate(out, g, 0);
-  cudaGraphDestroy(g);
-  if (err != cudaSuccess) return cz_fail(CZ_ERR_CUDA, "graph instantiate (range %d part %d) failed: %s", h, part, cudaGetErrorString(err));
-  return 0;
-}
-int build_graphs(cz_engine* e) {
-  for (int h = 0; h < e->n_ranges; ++h) {
-    int rc;
-    if ((rc = capture_part(e, h, 1, &e->g_pre[h])) || (rc = capture_part(e, h, 2, &e->g_tower[h])) || (rc = capture_part(e, h, 4, &e->g_post[h])))
-      return rc;
-  }
-  e->graphs_built = true;
-  return 0;
 }
 // launches per iteration of one range, for cz_launch_count (graph launches do not pass through launch_ok)
 int launches_per_iteration(cz_engine* e) { return 3 + cznn::nn_launches_per_forward(e->nn); }
 
 int search_graph_loop(cz_engine* e) {
+  const int prof = cznn::nn_profiling(e->nn) ? 1 : 0;
   CZ_LAUNCH(k_loop_reset, 1, 1, 0, e->stream, e->d);
-  e->h_flags[0] = 0; e->h_flags[1] = 1;
-  const bool prof = cznn::nn_profiling(e->nn);
-  if (e->graphs_built && e->g_while && !prof) {
-    // the whole loop is one graph launch (WHILE conditional node): the device iterates until no range has work left
-    if (cudaGraphLaunch(e->g_while, e->stream) != cudaSuccess)
-      return cz_fail(CZ_ERR_CUDA, "cz_search: WHILE graph launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-    if (cudaStreamSynchronize(e->stream) != cudaSuccess) return cz_fail(CZ_ERR_CUDA, "cz_search: device failure in the loop graph");
-    e->launches += (uint64_t)e->h_flags[0] * ((uint64_t)e->n_ranges * launches_per_iteration(e) + 1);
-    const char* m;
-    if (czrt_last_error(&m)) return cz_fail(CZ_ERR_CUDA, "cz_search: %s", m);
-    return 0;
+  if (!e->g_while[prof]) {
+    // The first search of each form runs its first iteration as plain launches: it loads every kernel and sets their
+    // attributes (neither may happen inside a stream capture) and is otherwise the same work.  The WHILE graph is captured
+    // right after it and runs the rest; its body always runs once, and an iteration with no work changes nothing.
+    int rc;
+    if ((rc = enqueue_iteration(e, nullptr)) || (rc = build_while_graph(e, prof))) return rc;
   }
-  const int kDepth = e->cfg.n_games * e->cfg.leaves_per_round >= 1024 ? 4 : 2;   // iterations the host may run ahead of the last one it saw finish
-  int launched = 0;
-  for (;;) {
-    for (int h = 0; h < e->n_ranges; ++h) {
-      if (!e->graphs_built) {
-        // The engine's very first iteration runs as plain launches: it loads every kernel and sets their attributes (neither
-        // may happen inside a stream capture) and is otherwise the same work; the graphs are captured right after it.
-        int rc;
-        if ((rc = enqueue_part(e, h, 1))) return rc;
-        if (prof) cznn::nn_prof_begin(e->nn, -1.0);
-        rc = enqueue_part(e, h, 2);
-        if (prof) cznn::nn_prof_end(e->nn);
-        if (rc || (rc = enqueue_part(e, h, 4))) return rc;
-      } else {
-        if (cudaGraphLaunch(e->g_pre[h], e->stream) != cudaSuccess) return cz_fail(CZ_ERR_CUDA, "cz_search: graph launch failed: %s", cudaGetErrorString(cudaGetLastError()));
-        if (prof) cznn::nn_prof_begin(e->nn, -1.0);
-        cudaGraphLaunch(e->g_tower[h], e->stream);
-        if (prof) cznn::nn_prof_end(e->nn);
-        cudaGraphLaunch(e->g_post[h], e->stream);
-      }
-    }
-    if (!e->graphs_built) {
-      int rc = build_graphs(e);
-      if (!rc) rc = build_while_graph(e);
-      if (rc) return rc;
-    }
-    ++launched;
-    e->launches += (uint64_t)e->n_ranges * launches_per_iteration(e) + 1;
-
-    // wait until fewer than kDepth iterations are outstanding, then look at the newest report
-    int done;
-    unsigned spins = 0;
-    while (launched - (done = e->h_flags[0]) >= kDepth) {
-      if (++spins >= 1000000u) {                         // every ~second of spinning: is the device still working on it?
-        spins = 0;
-        const cudaError_t q = cudaStreamQuery(e->stream);
-        if (q != cudaSuccess && q != cudaErrorNotReady) return cz_fail(CZ_ERR_CUDA, "cz_search: %s", cudaGetErrorString(q));
-        if (q == cudaSuccess && e->h_flags[0] == done) return cz_fail(CZ_ERR_CUDA, "cz_search: the loop flag of iteration %d never arrived", done + 1);
-      }
-    }
-    if (done > 0 && e->h_flags[1] == 0) break;           // an iteration finished with nothing left to do: the rest are no-ops
-  }
-  if (cudaStreamSynchronize(e->stream) != cudaSuccess) return cz_fail(CZ_ERR_CUDA, "cz_search: device failure");
-  const char* msg;
-  if (czrt_last_error(&msg)) return cz_fail(CZ_ERR_CUDA, "cz_search: %s", msg);
+  // the whole loop is one graph launch (WHILE conditional node): the device iterates until no range has work left
+  if (cudaGraphLaunch(e->g_while[prof], e->stream) != cudaSuccess)
+    return cz_fail(CZ_ERR_CUDA, "cz_search: WHILE graph launch failed: %s", cudaGetErrorString(cudaGetLastError()));
+  if (cudaStreamSynchronize(e->stream) != cudaSuccess) return cz_fail(CZ_ERR_CUDA, "cz_search: device failure in the loop graph");
+  e->launches += (uint64_t)*e->h_iters * ((uint64_t)e->n_ranges * launches_per_iteration(e) + 1);
+  const char* m;
+  if (czrt_last_error(&m)) return cz_fail(CZ_ERR_CUDA, "cz_search: %s", m);
   return 0;
 }
 }  // namespace
@@ -1010,17 +917,7 @@ int cz_nn_profile(cz_engine* e, int enable, double* ms, uint64_t* launches, doub
 #else
   if (!e || !e->nn) return cz_fail(CZ_ERR_STATE, "cz_nn_profile: engine has no network");
   cznn::nn_profile(e->nn, enable != 0);
-  double fl = 0.0;
-  const int rc = cznn::nn_profile_read(e->nn, ms, launches, &fl);      // synchronises the stream
-  if (rc) return rc;
-  // launches whose batch size only the device knew: positions evaluated by the loop since the last read
-  unsigned long long pos = 0;
-  czrt_copy(&pos, e->d.counters, sizeof(pos), e->stream);
-  if (czrt_sync(e->stream)) return cz_fail(CZ_ERR_CUDA, "cz_nn_profile: device failure");
-  fl += (double)(pos - e->prof_pos0) * cznn::nn_tower_flops_per_position(e->nn);
-  e->prof_pos0 = pos;
-  if (flops) *flops = fl;
-  return 0;
+  return cznn::nn_profile_read(e->nn, ms, launches, flops);           // synchronises the stream
 #endif
 }
 

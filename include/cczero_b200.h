@@ -233,10 +233,10 @@ int cz_search_more(cz_engine* e, int32_t n_sims);
  * per-game read position is kept.  Stream-ordered. */
 int cz_set_noise_table(cz_engine* e, const double* noise_dev, int64_t noise_stride);
 /* Whole search with the built-in network as evaluator (needs cz_nn_set_weights).  Device-driven: every wave / evaluation /
- * apply iteration is a fixed-shape sequence of launches whose batch size is a device integer, captured as CUDA graphs.  A
+ * apply iteration is a fixed-shape sequence of launches whose batch size is a device integer, captured as a CUDA graph.  A
  * search is one launch of a graph whose WHILE node repeats the iteration until no game has work left.  The engine's first
- * search runs one iteration as plain launches, captures the graphs, and runs the rest as three sub-graphs per iteration while
- * the host polls a flag in mapped memory; so does every search while cz_nn_profile is on (events bracket the tower).
+ * search runs one iteration as plain launches, captures the graph and launches it for the rest; so does the first search
+ * with cz_nn_profile on, which has a graph of its own (the same iteration with the tower bracketed by two timestamp kernels).
  * Synchronises once, at the end. */
 int cz_search(cz_engine* e, const cz_root_opts* opts);
 /* The loop of cz_search alone: run the simulations cz_search_begin / cz_search_more queued, built-in network as evaluator.
@@ -360,9 +360,10 @@ int cz_nn_forward(cz_engine* e, const float* planes_dev, int32_t batch, float* p
 /* Same from packed boards (plane encoding fused into the first convolution); with use_history every position is two
  * consecutive records: the board and the history board (all empty = zero planes). */
 int cz_nn_forward_boards(cz_engine* e, const uint8_t* boards_dev, int32_t batch, float* policy_dev, float* value_dev);
-/* CUDA-event timing of the residual-tower tensor-core launches (the dominant kernel): switches the
- * bracketing on/off and returns + clears what accumulated since the last call: device milliseconds,
- * launches and algorithmic FLOPs (2*90*9*C*C per position per launch).  Synchronises. */
+/* Timing of the residual-tower tensor-core launches (the dominant kernel): while on, every network forward (cz_search's
+ * included) brackets its tower with two one-thread kernels that read the device's %globaltimer.  Switches the bracketing
+ * on/off and returns + clears what accumulated since the last call: device milliseconds, launches and algorithmic FLOPs
+ * (2*90*9*C*C per position per launch, positions as counted on the device).  Synchronises. */
 int cz_nn_profile(cz_engine* e, int enable, double* ms, uint64_t* launches, double* flops);
 /* Kernel launches issued by this engine since creation (bench.py "gpu_launches"). */
 int cz_launch_count(cz_engine* e, uint64_t* n);

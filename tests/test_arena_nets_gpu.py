@@ -35,11 +35,11 @@ def _same(a, b):
     return a["moves"] == b["moves"] and a["p"] == b["p"] and a["n"] == b["n"] and a["w"] == b["w"]
 
 
-@pytest.mark.parametrize("profiled", [False, True], ids=["while_graph", "sub_graphs"])
+@pytest.mark.parametrize("profiled", [False, True], ids=["while_graph", "profiled_graph"])
 def test_arena_slot_ranges_search_with_their_own_network(cuda_lib, profiled):
-    """Two searches per engine: the first runs as plain launches and captures the graphs; the second runs as one WHILE-graph
-    launch, or with cz_nn_profile on as the sub-graph loop.  A third search after net 1 is reloaded with net 0's weights
-    checks that the captured graphs see a reload."""
+    """Two searches per engine: the first runs its first iteration as plain launches, captures the WHILE graph and launches it;
+    the second is one launch of that graph (with cz_nn_profile on, the profiled graph).  A third search after net 1 is
+    reloaded with net 0's weights checks that the captured graph sees a reload."""
     wa, wb = _weights(1), _weights(2)
     positions = [[osenv.INIT_STATE] * (N_SLOTS // 2) + sc.midgame_states(N_SLOTS // 2, 3),
                  sc.midgame_states(N_SLOTS, 4)]
