@@ -331,6 +331,23 @@ CZ_D void flip_only(const uint8_t* in, uint8_t* out) {
   czs::syncwarp();
 }
 
+// Left-right mirror across the central file (x -> 8 - x): square y*9+x goes to y*9+(8-x), the 6 pad bytes are copied.
+// The rules are symmetric under it and boards are mover-relative, so it commutes with step_flip.  in == out is allowed.
+CZ_D void mirror_board(const uint8_t* in, uint8_t* out) {
+  uint8_t v[3];
+  for (int j = 0; j < 3; ++j) {
+    const int sq = j * 32 + czs::lane();
+    v[j] = sq < BOARD_STRIDE ? in[sq] : (uint8_t)0;
+  }
+  czs::syncwarp();
+  for (int j = 0; j < 3; ++j) {
+    const int sq = j * 32 + czs::lane();
+    if (sq < NSQ) out[sq + 8 - 2 * (sq % 9)] = v[j];
+    else if (sq < BOARD_STRIDE) out[sq] = v[j];
+  }
+  czs::syncwarp();
+}
+
 CZ_D void copy_board(const uint8_t* in, uint8_t* out) {
   for (int j = 0; j < 3; ++j) {
     const int sq = j * 32 + czs::lane();

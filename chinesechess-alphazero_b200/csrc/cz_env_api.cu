@@ -99,6 +99,16 @@ CZ_KERNEL(k_env_keys)(const uint8_t* boards, int n, uint64_t* keys) {
   if (czs::lane() == 0) { keys[2 * i] = k0; keys[2 * i + 1] = k1; }
 }
 
+// flags NULL: every row mirrored; otherwise row i is mirrored where flags[i] != 0 and copied where it is 0.
+CZ_KERNEL(k_env_mirror)(const uint8_t* boards, const uint8_t* flags, int n, uint8_t* out) {
+  const int i = czs::block_idx() * czs::warps_per_block() + czs::warp_in_block();
+  if (i >= n) return;
+  EnvWarpSmem* sm = my_smem();
+  load_board(boards + (size_t)i * BOARD_STRIDE, sm->board);
+  if (!flags || flags[i]) mirror_board(sm->board, sm->board);
+  store_board(sm->board, out + (size_t)i * BOARD_STRIDE);
+}
+
 int finish_launch(const char* what) {
   const char* msg;
   const int e = czrt_last_error(&msg);
@@ -156,6 +166,13 @@ int cz_env_keys(const uint8_t* boards, int n, uint64_t* keys, void* stream) {
   return finish_launch("cz_env_keys");
 }
 
+int cz_env_mirror(const uint8_t* boards, const uint8_t* flags, int n, uint8_t* out, void* stream) {
+  if (n < 0 || (n && (!boards || !out))) return cz_fail(CZ_ERR_ARG, "cz_env_mirror: bad argument");
+  if (n == 0) return CZ_OK;
+  CZ_ENV_LAUNCH(k_env_mirror, n, (cz_stream_t)stream, boards, flags, n, out);
+  return finish_launch("cz_env_mirror");
+}
+
 // create_action_labels (environment/lookup_tables.py:62-132): per source square the same-row,
 // same-column and knight-jump destinations, then the fixed advisor and elephant moves.
 int cz_action_labels(char* labels, int16_t* lut) {
@@ -191,6 +208,22 @@ int cz_action_labels(char* labels, int16_t* lut) {
       "0729", "4729", "4769", "8769", "0725", "4725", "4765", "8765"};
   for (const char* s : fixed) add(s[0] - '0', s[1] - '0', s[2] - '0', s[3] - '0');
   if (cnt != CZ_N_LABELS) return cz_fail(CZ_ERR_STATE, "cz_action_labels: built %d labels", cnt);
+  return CZ_OK;
+}
+
+// M[l] = label of l's move reflected across the central file, built from cz_action_labels' strings and table.
+int cz_mirror_labels(int16_t* m) {
+  if (!m) return cz_fail(CZ_ERR_ARG, "cz_mirror_labels: NULL output");
+  char labels[CZ_N_LABELS * 4];
+  int16_t lut[8100];
+  const int rc = cz_action_labels(labels, lut);
+  if (rc) return rc;
+  for (int l = 0; l < CZ_N_LABELS; ++l) {
+    const char* s = labels + l * 4;
+    const int x0 = 8 - (s[0] - '0'), y0 = s[1] - '0', x1 = 8 - (s[2] - '0'), y1 = s[3] - '0';
+    m[l] = lut[(y0 * 9 + x0) * 90 + (y1 * 9 + x1)];
+    if (m[l] < 0) return cz_fail(CZ_ERR_STATE, "cz_mirror_labels: label %d has no mirror", l);
+  }
   return CZ_OK;
 }
 

@@ -428,17 +428,35 @@ __global__ void __launch_bounds__(256) k_softmax(const float* __restrict__ logit
 
 // Integrated search: softmax probabilities of the LEGAL moves of every leaf only (player.py:272-284 reads nothing else of the
 // policy vector).  labels [n][CZ_MAX_MOVES] int16 (-1 = the move has no label), counts [n]; out [n][CZ_MAX_MOVES] f32.  Warp per leaf.
+// kMirror (cz_config.eval_mirror): rows n..2n-1 are the leaves' mirrors; the prior is 0.5 * (p_leaf[lab] + p_{n+leaf}[M lab])
+// and value[leaf] = 0.5 * (value2[leaf] + value2[n + leaf]), each sum and product rounded once.
+template <bool kMirror>
 __global__ void __launch_bounds__(128) k_legal_priors(const float* __restrict__ logits, int ldl, const float2* __restrict__ stats, int n_tiles,
                                                        const int16_t* __restrict__ labels, const int32_t* __restrict__ counts,
-                                                       const int* __restrict__ n_dev, float* __restrict__ out) {
+                                                       const int* __restrict__ n_dev, float* __restrict__ out,
+                                                       const int16_t* __restrict__ mirror_lut, const float* __restrict__ value2,
+                                                       float* __restrict__ value) {
   const int leaf = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (leaf >= __ldg(n_dev)) return;
+  const int n = __ldg(n_dev);
+  if (leaf >= n) return;
   const RowStat rs = combine_stats(stats + (size_t)leaf * n_tiles, n_tiles);
   const float* l = logits + (size_t)leaf * ldl;
+  RowStat rm{};
+  const float* lm = nullptr;
+  if (kMirror) {
+    rm = combine_stats(stats + (size_t)(n + leaf) * n_tiles, n_tiles);
+    lm = logits + (size_t)(n + leaf) * ldl;
+    if (lane == 0) value[leaf] = __fmul_rn(0.5f, __fadd_rn(value2[leaf], value2[n + leaf]));
+  }
   const int L = counts[leaf];
   for (int i = lane; i < L; i += 32) {
     const int lab = labels[(size_t)leaf * CZ_MAX_MOVES + i];
-    out[(size_t)leaf * CZ_MAX_MOVES + i] = lab >= 0 ? policy_prob(l[lab], rs) : 0.f;
+    float p = 0.f;
+    if (lab >= 0) {
+      p = policy_prob(l[lab], rs);
+      if (kMirror) p = __fmul_rn(0.5f, __fadd_rn(p, policy_prob(lm[__ldg(mirror_lut + lab)], rm)));
+    }
+    out[(size_t)leaf * CZ_MAX_MOVES + i] = p;
   }
 }
 __global__ void k_set_int(int* p, int v) { *p = v; }
@@ -882,13 +900,21 @@ int nn_forward_planes(NnRuntime* r, int net, const float* planes, int batch, flo
 // The search's evaluation step: up to n_max leaves (actual count *n_dev), boards + legal-move labels in, value [n] and the
 // softmax probabilities of the legal moves [n][CZ_MAX_MOVES] out.  Fixed launch shapes: safe to capture into a CUDA graph.
 int nn_forward_leaves(NnRuntime* r, int net, const uint8_t* boards, int n_max, const int* n_dev, const int16_t* labels,
-                      const int32_t* label_counts, float* legal_p, float* value) {
+                      const int32_t* label_counts, float* legal_p, float* value, const int16_t* mirror_lut, float* value2) {
   const NetWeights* w = ready_net(r, net);
   if (!w) return CZ_ERR_STATE;
-  if (n_max > r->max_batch) return cz_fail(CZ_ERR_ARG, "nn_forward_leaves: %d leaves > max batch %d", n_max, r->max_batch);
-  const int rc = forward_tower(r, *w, boards, n_max, n_dev, value);
+  const bool mirror = mirror_lut != nullptr;
+  const int rows = mirror ? 2 * n_max : n_max;
+  if (rows > r->max_batch) return cz_fail(CZ_ERR_ARG, "nn_forward_leaves: %d rows > max batch %d", rows, r->max_batch);
+  if (mirror && !value2) return cz_fail(CZ_ERR_ARG, "nn_forward_leaves: the mirror form needs its value scratch");
+  const int rc = forward_tower(r, *w, boards, rows, mirror ? n_dev + 2 : n_dev, mirror ? value2 : value);
   if (rc) return rc;
-  k_legal_priors<<<(n_max + 3) / 4, 128, 0, r->stream>>>(r->logits, kPolN, r->stats, kPolN / 256, labels, label_counts, n_dev, legal_p);
+  if (mirror)
+    k_legal_priors<true><<<(n_max + 3) / 4, 128, 0, r->stream>>>(r->logits, kPolN, r->stats, kPolN / 256, labels, label_counts, n_dev,
+                                                                 legal_p, mirror_lut, value2, value);
+  else
+    k_legal_priors<false><<<(n_max + 3) / 4, 128, 0, r->stream>>>(r->logits, kPolN, r->stats, kPolN / 256, labels, label_counts, n_dev,
+                                                                  legal_p, nullptr, nullptr, nullptr);
   r->launches++;
   CZ_CUDA(cudaGetLastError());
   return 0;

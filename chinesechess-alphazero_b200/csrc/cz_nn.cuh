@@ -24,8 +24,12 @@ int nn_forward_planes(NnRuntime*, int net, const float* planes_dev, int batch, f
 // shapes, capturable into a CUDA graph).  labels_dev [n][CZ_MAX_MOVES] int16 = action label of every legal move (-1: none),
 // label_counts_dev [n]; legal_p_dev [n][CZ_MAX_MOVES] f32 gets the softmax probability of exactly those labels — bit for bit
 // the numbers nn_forward_boards writes at those indices of its [n][2086] vector.
+// Mirror form (mirror_lut_dev = cz_mirror_labels on the device, value2_dev [2 * n_max] scratch): boards_dev holds the n
+// leaves and then their mirrors, n_dev[2] = 2 * n_dev[0] rows are evaluated, and leaf i gets
+// 0.5 * (p_i[lab] + p_{n+i}[M lab]) and 0.5 * (v_i + v_{n+i}), each sum and product rounded once in fp32.
 int nn_forward_leaves(NnRuntime*, int net, const uint8_t* boards_dev, int n_max, const int* n_dev, const int16_t* labels_dev,
-                      const int32_t* label_counts_dev, float* legal_p_dev, float* value_dev);
+                      const int32_t* label_counts_dev, float* legal_p_dev, float* value_dev,
+                      const int16_t* mirror_lut_dev, float* value2_dev);
 bool nn_profiling(const NnRuntime*);
 // launches of one nn_forward_leaves, the two profiling stamps included while profiling is on
 int nn_launches_per_forward(const NnRuntime*);

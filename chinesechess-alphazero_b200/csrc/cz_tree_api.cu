@@ -117,14 +117,20 @@ __global__ void __launch_bounds__(1024) k_scan_block(EngineDev E, int gb, int ge
   }
 }
 #endif
-CZ_KERNEL(k_gather)(EngineDev E, int g0, int g1, uint8_t* dense, int16_t* labels, int32_t* nlab) {
+// mirror_tot (eval_mirror, device-driven loop): the range's totals slot; leaf j of the range is also written, mirrored, at
+// row totals[0] + j, and totals[2] = 2 * totals[0] is the row count the network reads.  Null: the plain form.
+CZ_KERNEL(k_gather)(EngineDev E, int g0, int g1, uint8_t* dense, int16_t* labels, int32_t* nlab, int32_t* mirror_tot) {
   const int g = g0 + my_game();
   if (g >= g1) return;
+  const int n_range = mirror_tot ? mirror_tot[0] : 0;
+  if (mirror_tot && g == g0 && czs::lane() == 0) mirror_tot[2] = 2 * n_range;
   const int n = E.n_leaf[g], off = E.leaf_off[g];
   for (int j = 0; j < n; ++j) {
     const uint8_t* s = E.leaf_board + ((size_t)g * E.K + j) * E.lb_stride;
     uint8_t* d = dense + (size_t)(off + j) * E.lb_stride;
     if (czs::lane() < E.lb_stride / 16) reinterpret_cast<uint4*>(d)[czs::lane()] = reinterpret_cast<const uint4*>(s)[czs::lane()];
+    if (mirror_tot)
+      for (int b = 0; b < E.lb_stride; b += BOARD_STRIDE) mirror_board(s + b, dense + (size_t)(n_range + off + j) * E.lb_stride + b);
     const int node = E.sim_leaf_node[(size_t)g * E.K + E.leaf_sim[(size_t)g * E.K + j]];
     const size_t ni = (size_t)g * E.ncap + node;
     const int L = (int)(E.node_meta[ni] & 0xff);
@@ -323,6 +329,8 @@ struct cz_engine {
   cz_root_info* root_info_dev;
   float* value_buf;                                         // [G*K] values of the built-in network (integrated search)
   float* legal_p;                                           // [G*K][MAX_MOVES] priors of the legal moves (integrated search)
+  float* value2;                                            // eval_mirror: [2*G*K] network values of the leaves and their mirrors
+  int16_t* mirror_lut;                                      // eval_mirror: [CZ_N_LABELS] cz_mirror_labels
   uint8_t* board_stage;                                     // [G][96] staging for reset / set_root
   int32_t* stat_n; uint16_t* stat_mv; int32_t* stat_cnt;    // staging for cz_get_root_stats
   int32_t* sims_stage;                                      // [G] staging for cz_set_game_sims
@@ -376,7 +384,9 @@ size_t carve(cz_engine* e, uint8_t* base) {
   d.resume_sim = cv.take<int32_t>(G * K); d.n_resume = cv.take<int32_t>(G);
   d.park_sim = cv.take<int32_t>(G * K); d.park_node = cv.take<int32_t>(G * K); d.n_park = cv.take<int32_t>(G);
   d.leaf_off = cv.take<int32_t>(G); d.totals = cv.take<int32_t>(8);
-  d.leaf_dense = cv.take<uint8_t>(G * K * d.lb_stride);
+  // eval_mirror: 2*G*K rows, range h owns [2*gb*K, 2*ge*K): its n leaves, then their mirrors (k_gather)
+  const size_t dense_rows = (c.eval_mirror ? 2 : 1) * G * K;
+  d.leaf_dense = cv.take<uint8_t>(dense_rows * d.lb_stride);
   d.leaf_labels = cv.take<int16_t>(G * K * MAX_MOVES); d.leaf_nlab = cv.take<int32_t>(G * K);
   d.loop_iter = cv.take<int32_t>(4);
   d.noise_ref = cv.take<NoiseRef>(1);
@@ -399,6 +409,12 @@ size_t carve(cz_engine* e, uint8_t* base) {
   } else {
     e->value_buf = nullptr; e->legal_p = nullptr;
   }
+  if (c.eval_mirror) {
+    e->value2 = cv.take<float>(2 * G * K);
+    e->mirror_lut = cv.take<int16_t>(CZ_N_LABELS);
+  } else {
+    e->value2 = nullptr; e->mirror_lut = nullptr;
+  }
   visits_carve(d.sp, cv, c);
   return cv.off + 1024;
 }
@@ -418,6 +434,9 @@ int check_cfg(const cz_config* c) {
   if (c->arena && (c->n_games % 2)) return cz_fail(CZ_ERR_ARG, "cz_config: arena mode needs an even number of slots (two per game)");
   // the arena's records are scored, never trained on (evaluator.py), and its two slots per game would need a shared staging
   if (c->arena && c->record_visits) return cz_fail(CZ_ERR_ARG, "cz_config: record_visits is for self-play engines, not arena ones");
+  if (c->eval_mirror != 0 && c->eval_mirror != 1) return cz_fail(CZ_ERR_ARG, "cz_config: eval_mirror must be 0 or 1");
+  // the mirrored evaluation is the engine's own network run twice; an external evaluator gets the leaves as they are
+  if (c->eval_mirror && c->nn_filters == 0) return cz_fail(CZ_ERR_ARG, "cz_config: eval_mirror needs the engine's own network (nn_filters > 0)");
   return 0;
 }
 
@@ -436,6 +455,9 @@ void init_board(uint8_t* b) {
     b[y * 9 + x++] = code;
   }
 }
+
+// rows of the network's batch: the leaves of one search round, and with eval_mirror their mirrors too
+int nn_max_batch(const cz_config* c) { return (c->eval_mirror ? 2 : 1) * c->n_games * c->leaves_per_round; }
 
 int launch_ok(cz_engine* e, const char* what, int n = 1) {
   e->launches += n;
@@ -461,7 +483,7 @@ int cz_workspace_bytes(const cz_config* cfg, uint64_t* bytes) {
   size_t n = carve(&tmp, nullptr);
 #if !defined(CZ_EMUL)
   if (cfg->nn_filters > 0)
-    n += cznn::nn_workspace_bytes(cfg->nn_filters, cfg->nn_blocks, cfg->nn_value_fc, cfg->n_games * cfg->leaves_per_round, cfg->arena ? 2 : 1,
+    n += cznn::nn_workspace_bytes(cfg->nn_filters, cfg->nn_blocks, cfg->nn_value_fc, nn_max_batch(cfg), cfg->arena ? 2 : 1,
                                   cfg->nn_policy_channels, cfg->nn_value_channels) + 4096;
 #endif
   *bytes = n;
@@ -517,12 +539,17 @@ int cz_create(const cz_config* cfg, void* workspace, uint64_t workspace_bytes, v
   uint8_t ib[BOARD_STRIDE];
   init_board(ib);
   czrt_copy(e->init_board_dev, ib, BOARD_STRIDE, e->stream);
+  if (e->mirror_lut) {
+    int16_t m[CZ_N_LABELS];
+    cz_mirror_labels(m);
+    czrt_copy(e->mirror_lut, m, sizeof(m), e->stream);
+  }
   czrt_memset(d.counters, 0, 8 * sizeof(unsigned long long), e->stream);
   czrt_memset(d.stat, 0, (size_t)cfg->n_games * 4 * sizeof(unsigned long long), e->stream);
   czrt_sync(e->stream);
 #if !defined(CZ_EMUL)
   if (cfg->nn_filters > 0) {
-    const int maxb = cfg->n_games * cfg->leaves_per_round;
+    const int maxb = nn_max_batch(cfg);
     e->nn_bytes = cznn::nn_workspace_bytes(cfg->nn_filters, cfg->nn_blocks, cfg->nn_value_fc, maxb, cfg->arena ? 2 : 1,
                                            cfg->nn_policy_channels, cfg->nn_value_channels);
     uint8_t* nnws = e->ws + ((used + 4095) & ~(size_t)4095);
@@ -651,7 +678,7 @@ int cz_search_wave(cz_engine* e, int32_t* n_leaves, int32_t* any_active) {
   const int G = e->cfg.n_games;
   RANGE_LAUNCH(e, e->stream, 0, G, k_wave, e->d, 0, G);
   CZ_LAUNCH(k_scan, 1, 1, 0, e->stream, e->d, 0, G, 0);
-  RANGE_LAUNCH(e, e->stream, 0, G, k_gather, e->d, 0, G, e->d.leaf_dense, e->d.leaf_labels, e->d.leaf_nlab);
+  RANGE_LAUNCH(e, e->stream, 0, G, k_gather, e->d, 0, G, e->d.leaf_dense, e->d.leaf_labels, e->d.leaf_nlab, (int32_t*)nullptr);
   if (launch_ok(e, "cz_search_wave", 3)) return CZ_ERR_CUDA;
   int32_t t[4];
   czrt_copy(t, e->d.totals, sizeof(t), e->stream);
@@ -718,7 +745,7 @@ Range range_of(cz_engine* e, int h) {
   Range r;
   r.gb = h == 0 ? 0 : mid; r.ge = h == 0 ? mid : G;
   const size_t off = (size_t)r.gb * K;
-  r.dense = e->d.leaf_dense + off * e->d.lb_stride;
+  r.dense = e->d.leaf_dense + (e->cfg.eval_mirror ? 2 : 1) * off * e->d.lb_stride;
   r.labels = e->d.leaf_labels + off * MAX_MOVES; r.nlab = e->d.leaf_nlab + off;
   r.legal_p = e->legal_p + off * MAX_MOVES; r.value = e->value_buf + off;
   return r;
@@ -731,8 +758,11 @@ int enqueue_iteration(cz_engine* e, const cudaGraphConditionalHandle* cond) {
     const int n_max = (r.ge - r.gb) * e->cfg.leaves_per_round;
     RANGE_LAUNCH(e, e->stream, r.gb, r.ge, k_apply_wave, e->d, r.gb, r.ge, (const float*)r.legal_p, (const float*)r.value);
     k_scan_block<<<1, 1024, 0, e->stream>>>(e->d, r.gb, r.ge, h);
-    RANGE_LAUNCH(e, e->stream, r.gb, r.ge, k_gather, e->d, r.gb, r.ge, r.dense, r.labels, r.nlab);
-    const int rc = cznn::nn_forward_leaves(e->nn, e->cfg.arena ? h : 0, r.dense, n_max, e->d.totals + 4 * h, r.labels, r.nlab, r.legal_p, r.value);
+    int32_t* tot = e->d.totals + 4 * h;
+    const bool mirror = e->cfg.eval_mirror != 0;
+    RANGE_LAUNCH(e, e->stream, r.gb, r.ge, k_gather, e->d, r.gb, r.ge, r.dense, r.labels, r.nlab, mirror ? tot : (int32_t*)nullptr);
+    const int rc = cznn::nn_forward_leaves(e->nn, e->cfg.arena ? h : 0, r.dense, n_max, tot, r.labels, r.nlab, r.legal_p, r.value,
+                                           mirror ? e->mirror_lut : nullptr, mirror ? e->value2 + 2 * (size_t)r.gb * e->cfg.leaves_per_round : nullptr);
     if (rc) return rc;
   }
   CZ_LAUNCH(k_loop_flag, 1, 1, 0, e->stream, e->d, e->n_ranges, e->d_iters, cond ? (unsigned long long)*cond : 0ULL, cond ? 1 : 0);

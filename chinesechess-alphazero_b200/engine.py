@@ -23,7 +23,7 @@ class Engine:
                  nn_filters=0, nn_blocks=0, nn_value_fc=256, c_puct=1.5, noise_eps=0.15, dirichlet_alpha=0.2,
                  tau_decay_rate=0.9, resign_threshold=-0.98, enable_resign_rate=0.5, min_resign_turn=40, seed=0, rank=0, nn_fp32_skip=None, arena=False,
                  use_history=False, game_quota=0, playouts=None, nn_policy_channels=0, nn_value_channels=0,
-                 record_visits=False):
+                 record_visits=False, eval_mirror=False):
         self.lib = lib or get_lib()
         if device is None:
             device = 'cuda' if self.lib.is_cuda else 'cpu'
@@ -56,6 +56,8 @@ class Engine:
         cfg.nn_policy_channels, cfg.nn_value_channels = int(nn_policy_channels or 0), int(nn_value_channels or 0)
         cfg.record_visits = 1 if record_visits else 0   # every ply's root visit counts go with the records (drain_records)
         self.record_visits = bool(record_visits)
+        # the built-in network evaluates every leaf and its left-right mirror and averages them (cz_config.eval_mirror)
+        cfg.eval_mirror = 1 if eval_mirror else 0
         self.use_history = bool(use_history)
         self.in_planes = 28 if use_history else 14
         self.cfg = cfg

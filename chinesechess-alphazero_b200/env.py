@@ -123,6 +123,7 @@ class StaticEnv:
         raw = labels.raw.decode()
         self.labels = [raw[i * 4:i * 4 + 4] for i in range(N_LABELS)]
         self.label_lut = lut
+        self._mirror_labels = self._mirror_labels_dev = None
         self.INIT_STATE = INIT_STATE
 
     # ---- plumbing
@@ -178,6 +179,31 @@ class StaticEnv:
         keys = torch.empty((n, 2), dtype=torch.int64, device=self.device)
         self.lib.call("cz_env_keys", _ptr(boards), n, _ptr(keys), self._stream())
         return keys
+
+    @property
+    def mirror_labels(self):
+        """int16 [2086]: the label of each label's move reflected across the central file (cz_mirror_labels)."""
+        if self._mirror_labels is None:
+            m = np.empty(N_LABELS, dtype=np.int16)
+            self.lib.call("cz_mirror_labels", C.c_void_p(m.ctypes.data))
+            self._mirror_labels = m
+        return self._mirror_labels
+
+    def mirror(self, boards, flags=None):
+        """Boards reflected across the central file (x -> 8 - x).  flags: optional uint8/bool [n] tensor on the device,
+        rows with flag 0 come back unchanged."""
+        n = boards.shape[0]
+        out = torch.empty_like(boards)
+        if flags is not None:
+            flags = flags.to(torch.uint8).contiguous()
+        self.lib.call("cz_env_mirror", _ptr(boards), _ptr(flags), n, _ptr(out), self._stream())
+        return out
+
+    def mirror_policy(self, policy, flags):
+        """Policy rows [n][2086] of mirrored positions: row'[l] = row[M l] where flags (bool [n] tensor) is set."""
+        if self._mirror_labels_dev is None:
+            self._mirror_labels_dev = self.to_dev(self.mirror_labels.astype(np.int64))
+        return torch.where(flags.bool().unsqueeze(1), policy.index_select(1, self._mirror_labels_dev), policy)
 
     def moves_tensor(self, moves):
         return self.to_dev(np.array([move_to_u16(m) for m in moves], dtype=np.uint16).view(np.int16))

@@ -37,9 +37,10 @@ def tally_games(results):
 
 class EvaluateWorker:
     def __init__(self, config, model_bt, model_ng, n_games=None, concurrent_games=None, lib=None, device=None, seed=0,
-                 playouts=(8, 12)):
+                 playouts=(8, 12), eval_mirror=False):
         """playouts: every game draws `randint(lo, hi) * 100` simulations per move when it starts (evaluator.py:153-154);
-        None = config.play.simulation_num_per_move for every game."""
+        None = config.play.simulation_num_per_move for every game.  eval_mirror: each side's network averages every leaf
+        and its left-right mirror."""
         self.config = config
         pc, mc = config.play, config.model
         self.n_games = n_games or config.eval.game_num * pc.max_processes
@@ -52,7 +53,7 @@ class EvaluateWorker:
             noise_eps=pc.noise_eps, dirichlet_alpha=getattr(pc, "dirichlet_alpha", 0.2), tau_decay_rate=pc.tau_decay_rate,
             enable_resign_rate=0.0, max_game_length=pc.max_game_length, max_nodes_per_game=max(4096, 16 * sims_max),
             seed=seed, arena=True, **engine_net_kwargs(mc),
-            game_quota=self.n_games, playouts=playouts)   # exactly the games 0 .. n_games-1, each played to its end
+            game_quota=self.n_games, playouts=playouts, eval_mirror=eval_mirror)   # exactly the games 0 .. n_games-1, each played to its end
         self.engine.set_weights(model_bt.torch_weights(), net=0)
         self.engine.set_weights(model_ng.torch_weights(), net=1)
         self.engine.reset()
@@ -77,7 +78,7 @@ class EvaluateWorker:
         self.engine.close()
 
 
-def start(config, model_bt=None, model_ng=None):
+def start(config, model_bt=None, model_ng=None, eval_mirror=False):
     """evaluator.py:28-82."""
     from .model import CChessModel
     rc = config.resource
@@ -89,7 +90,7 @@ def start(config, model_bt=None, model_ng=None):
         model_ng = CChessModel(config)
         if not model_ng.load(rc.next_generation_config_path, rc.next_generation_weight_path):
             raise FileNotFoundError("next generation model not found")
-    worker = EvaluateWorker(config, model_bt, model_ng)
+    worker = EvaluateWorker(config, model_bt, model_ng, eval_mirror=eval_mirror)
     total_score, rw, rd, rf, bw, bd, bf = worker.start()
     game_num = worker.n_games
     worker.close()

@@ -33,6 +33,7 @@ class CzConfig(C.Structure):
         ("seed", C.c_uint64), ("rank", C.c_int32), ("arena", C.c_int32), ("nn_fp32_skip", C.c_int32), ("use_history", C.c_int32),
         ("game_quota", C.c_int32), ("playouts_lo", C.c_int32), ("playouts_hi", C.c_int32),
         ("nn_policy_channels", C.c_int32), ("nn_value_channels", C.c_int32), ("record_visits", C.c_int32),
+        ("eval_mirror", C.c_int32),
     ]
 
 
@@ -85,12 +86,14 @@ _SIGS = {
     "cz_last_error": (C.c_char_p, []),
     "cz_build_is_cuda": (C.c_int, []),
     "cz_action_labels": (C.c_int, [_P, _P]),
+    "cz_mirror_labels": (C.c_int, [_P]),
     "cz_env_movegen": (C.c_int, [_P, C.c_int, _P, _P, _P]),
     "cz_env_done": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P]),
     "cz_env_step": (C.c_int, [_P, _P, C.c_int, _P, _P, _P]),
     "cz_env_encode_planes": (C.c_int, [_P, C.c_int, _P, _P]),
     "cz_env_check_catch": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, _P]),
     "cz_env_keys": (C.c_int, [_P, C.c_int, _P, _P]),
+    "cz_env_mirror": (C.c_int, [_P, _P, C.c_int, _P, _P]),
     "cz_sl_replay": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "cz_play_replay": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, _P, _P]),
     "cz_workspace_bytes": (C.c_int, [C.POINTER(CzConfig), C.POINTER(C.c_uint64)]),

@@ -21,6 +21,11 @@ trainer the same values.
 (self-play with `record_visits`, records.py): target[l] = float32(n_l / sum n), the AlphaZero target calc_policy builds
 (agent/player.py:375-406).  Plies without visits, such as the appended final king capture or older files, keep the
 one-hot of their move.  The default "move" is the reference's one-hot target (optimize.py:248).
+
+`augment="mirror"` trains on both orientations of the data: Xiangqi's rules and action labels are symmetric across the
+central file, so every epoch each training sample is reflected (planes along x, policy columns by the label mirror M)
+with probability 1/2, flags drawn from numpy's global RNG right after the epoch's shuffle.  The validation samples are
+never reflected, and without `augment` no flags are drawn, so the default path's random numbers are unchanged.
 """
 import os
 import shutil
@@ -38,8 +43,8 @@ from .records import (PlayGames, check_labels, expanding_data, get_game_data_fil
 logger = getLogger(__name__)
 
 
-def start(config, policy_target="move"):
-    return OptimizeWorker(config, policy_target=policy_target).start()
+def start(config, policy_target="move", augment=None):
+    return OptimizeWorker(config, policy_target=policy_target, augment=augment).start()
 
 
 def load_best_model_weight(model):
@@ -84,6 +89,26 @@ def validation_split(n, split=0.02):
     return np.arange(split_at), np.arange(split_at, n)
 
 
+def check_augment(augment):
+    if augment not in (None, "mirror"):
+        raise ValueError(f"augment must be None or 'mirror', not {augment!r}")
+    return augment
+
+
+def mirror_flags(augment, n):
+    """Per-sample reflection flags of one epoch (drawn only when augmenting, after the epoch's shuffle)."""
+    return np.random.randint(0, 2, n) if augment else None
+
+
+def mirror_batch(planes, policy, flags, mirror_labels):
+    """Host form of SlDataset.batch's reflection: flagged rows' planes reversed along x, policy columns permuted by M
+    (an involution, so row'[l] = row[M l]).  planes and policy are the batch's own copies and are changed in place."""
+    f = np.asarray(flags).astype(bool)
+    planes[f] = planes[f][..., ::-1]
+    policy[f] = policy[f][:, mirror_labels]
+    return planes, policy
+
+
 def make_batches(size, batch_size):
     """Keras _make_batches: ceil(size / batch_size) slices, the last one partial."""
     nb = int(np.ceil(size / float(batch_size)))
@@ -91,13 +116,15 @@ def make_batches(size, batch_size):
 
 
 class OptimizeWorker:
-    def __init__(self, config, env=None, trainer_factory=None, device=None, dataset=None, policy_target="move"):
+    def __init__(self, config, env=None, trainer_factory=None, device=None, dataset=None, policy_target="move",
+                 augment=None):
         """env: StaticEnv for replaying records (default: the CUDA rules kernels); trainer_factory(model, batch_size, device)
         builds the object whose step(planes, policy, value, lr) / validation_loss(...) / export() train (default
         train.Trainer).  dataset: "device" keeps the positions on env's device and hands `step` device tensors, "host"
         expands them into numpy arrays; the default is "device" with the built-in trainer and "host" with a
         trainer_factory.  policy_target: "move" (one-hot of the played move) or "visits" (the recorded visit
-        distribution where a ply has one)."""
+        distribution where a ply has one).  augment: None or "mirror" (each epoch, every training sample reflected
+        across the central file with probability 1/2)."""
         if dataset is None:
             dataset = "device" if trainer_factory is None else "host"
         if dataset not in ("device", "host"):
@@ -106,6 +133,7 @@ class OptimizeWorker:
         if policy_target not in ("move", "visits"):
             raise ValueError(f"policy_target must be 'move' or 'visits', not {policy_target!r}")
         self.policy_target = policy_target
+        self.augment = check_augment(augment)
         self.config = config
         self.model = None
         self.loaded_filenames = set()
@@ -186,10 +214,14 @@ class OptimizeWorker:
         for epoch in range(epochs):
             order = train_idx.copy()
             np.random.shuffle(order)
+            flags = mirror_flags(self.augment, len(order))
             losses = []
             for a, b in make_batches(len(order), batch_size):
                 ids = order[a:b]
-                losses.append(self.trainer.step(x[ids], policy[ids], value[ids], lr))
+                xb, pb = x[ids], policy[ids]
+                if flags is not None:
+                    xb, pb = mirror_batch(xb, pb, flags[a:b], self._env().mirror_labels)
+                losses.append(self.trainer.step(xb, pb, value[ids], lr))
             rec = {"epoch": epoch, "lr": lr, "loss": float(np.mean([l[0] for l in losses])) if losses else None}
             if len(val_idx):
                 rec["val_loss"] = self.trainer.validation_loss(x[val_idx], policy[val_idx], value[val_idx])[0]
@@ -209,9 +241,11 @@ class OptimizeWorker:
         for epoch in range(epochs):
             order = train_idx.copy()
             np.random.shuffle(order)
+            flags = mirror_flags(self.augment, len(order))
             losses = []
             for a, b in make_batches(len(order), batch_size):
-                losses.append(self.trainer.step(*data.batch(env, order[a:b], history), lr))
+                mirror = None if flags is None else flags[a:b]
+                losses.append(self.trainer.step(*data.batch(env, order[a:b], history, mirror), lr))
             rec = {"epoch": epoch, "lr": lr, "loss": float(np.mean([l[0] for l in losses])) if losses else None}
             if val is not None:
                 rec["val_loss"] = self.trainer.validation_loss(*val)[0]

@@ -53,7 +53,8 @@ class NodeView:
 class CChessPlayer:
     def __init__(self, config, search_tree=None, pipes=None, play_config=None, enable_resign=False, debugging=False,
                  uci=False, use_history=False, side=0, lib=None, device=None, weights=None, exact_noise=True,
-                 infinite_capacity=200000):
+                 infinite_capacity=200000, eval_mirror=False):
+        """eval_mirror: the built-in network's evaluations average each leaf and its left-right mirror (Engine)."""
         self.use_history = use_history          # 28 input planes (static_env.py:158-194, player.py:326-334)
         self.config = config
         self.play_config = play_config or config.play
@@ -93,7 +94,7 @@ class CChessPlayer:
             resign_threshold=getattr(pc, "resign_threshold", -1.0), min_resign_turn=getattr(pc, "min_resign_turn", 0),
             max_game_length=getattr(pc, "max_game_length", 100),
             max_nodes_per_game=max(4096, 8 * pc.simulation_num_per_move, (infinite_capacity + 64) if uci else 0),
-            use_history=use_history, **(engine_net_kwargs(mc) if (use_nn and mc) else {}))
+            use_history=use_history, eval_mirror=eval_mirror, **(engine_net_kwargs(mc) if (use_nn and mc) else {}))
         if use_nn:
             if weights is None:
                 raise ValueError("CChessPlayer without pipes needs `weights` (Keras-named tensors) for the built-in network")

@@ -33,7 +33,7 @@ def load_model(config):
 
 
 def start(config, games_per_process=128, max_games=None, flush_plies=8, lib=None, device=None, evaluate_planes=None,
-          record_visits=False):
+          record_visits=False, eval_mirror=False):
     """self_play.py:48-60.  The reference fans out over `max_processes` OS processes that share one prediction thread;
     here one process drives one GPU, and data parallelism is one process per GPU under `torchrun` (RANK / LOCAL_RANK /
     WORLD_SIZE in the environment): rank r plays its own `max_processes x games_per_process` concurrent games on GPU
@@ -41,14 +41,15 @@ def start(config, games_per_process=128, max_games=None, flush_plies=8, lib=None
     ranks all_gather their finished-game rings (NCCL over NVLink; gloo on CPU) and rank 0 decodes them and writes the
     reference's play-data files (worker/self_play.py:202-232): the other ranks never touch the disk.
     record_visits=True also writes every ply's root visit counts into the files (records.py), the target of
-    optimize's policy_target="visits".
+    optimize's policy_target="visits".  eval_mirror=True averages the network over every leaf and its left-right mirror.
     Returns the number of games stored by this launch (rank 0; the others return the same total)."""
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
     model, use_history = load_model(config) if rank == 0 or world == 1 else (None, None)
     if world == 1:
         worker = SelfPlayWorker(config, pipes=None, pid=0, use_history=use_history, model=model, lib=lib, device=device,
-                                concurrent_games=config.play.max_processes * games_per_process, record_visits=record_visits)
+                                concurrent_games=config.play.max_processes * games_per_process, record_visits=record_visits,
+                                eval_mirror=eval_mirror)
         return worker.start(max_games=max_games)
     import torch
     import torch.distributed as dist
@@ -68,7 +69,8 @@ def start(config, games_per_process=128, max_games=None, flush_plies=8, lib=None
             dist.barrier()
         worker = SelfPlayWorker(config, pipes=None, pid=rank, use_history=use_history, model=model, lib=lib, device=device,
                                 concurrent_games=config.play.max_processes * games_per_process, rank=rank,
-                                external_evaluator=evaluate_planes is not None, record_visits=record_visits)
+                                external_evaluator=evaluate_planes is not None, record_visits=record_visits,
+                                eval_mirror=eval_mirror)
         return worker.start_distributed(dist, world, max_games=max_games, flush_plies=flush_plies, evaluate_planes=evaluate_planes)
     finally:
         if created:
@@ -77,7 +79,8 @@ def start(config, games_per_process=128, max_games=None, flush_plies=8, lib=None
 
 class SelfPlayWorker:
     def __init__(self, config, pipes=None, pid=None, use_history=False, model=None, concurrent_games=None, lib=None,
-                 device=None, seed=0, rank=0, external_evaluator=False, engine_kwargs=None, record_visits=False):
+                 device=None, seed=0, rank=0, external_evaluator=False, engine_kwargs=None, record_visits=False,
+                 eval_mirror=False):
         self.config = config
         self.cur_pipes = pipes          # unused: evaluation happens inside the engine
         self.id = pid
@@ -98,7 +101,7 @@ class SelfPlayWorker:
             **dict(dict(max_nodes_per_game=max(4096, 24 * pc.simulation_num_per_move),
                         seed=seed, rank=rank, **({} if external_evaluator else engine_net_kwargs(mc)),
                         use_history=use_history,    # the game loop never passes `hist` (self_play.py:124): path history only
-                        record_visits=record_visits),
+                        record_visits=record_visits, eval_mirror=eval_mirror),
                    **(engine_kwargs or {})))
         if not external_evaluator:      # external evaluator: the leaves go to a caller-supplied function (CPU test tier)
             self.engine.set_weights(self.model.torch_weights())

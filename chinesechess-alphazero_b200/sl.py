@@ -10,6 +10,9 @@ reshuffles the training indices every epoch, the final partial batch is kept, an
 mode.  Deviations: a game whose records make the reference raise (a missing or duplicated turn row, a move naming no
 piece, an unparseable move) is skipped and counted instead of aborting the run; a 28-plane (history) network is
 rejected; TensorBoard callbacks are not built.
+
+`augment="mirror"` reflects each training sample across the central file with probability 1/2 every epoch, as
+OptimizeWorker does (optimize.py); the validation samples are never reflected.
 """
 from logging import getLogger
 from time import time
@@ -19,13 +22,13 @@ import numpy as np
 
 from . import sl_data as sd
 from .model import CChessModel, N_LABELS
-from .optimize import make_batches, validation_split
+from .optimize import check_augment, make_batches, mirror_flags, validation_split
 
 logger = getLogger(__name__)
 
 
-def start(config):
-    return SupervisedWorker(config).start()
+def start(config, augment=None):
+    return SupervisedWorker(config, augment=augment).start()
 
 
 def load_sl_best_model_weight(model):
@@ -41,10 +44,12 @@ def save_as_sl_best_model(model):
 class SupervisedWorker:
     LR = 1e-2                                      # sl.py:81 Adam(lr=1e-2)
 
-    def __init__(self, config, trainer_factory=None, device=None, lib=None):
+    def __init__(self, config, trainer_factory=None, device=None, lib=None, augment=None):
         """trainer_factory(model, batch_size, device, optimizer="adam") builds the object whose step / validation_loss /
-        export train (default train.Trainer); lib: the rules library (default the CUDA product)."""
+        export train (default train.Trainer); lib: the rules library (default the CUDA product); augment: None or
+        "mirror"."""
         self.config = config
+        self.augment = check_augment(augment)
         self.model = None
         self.dataset = None
         self.opt = None
@@ -120,9 +125,10 @@ class SupervisedWorker:
         for epoch in range(epochs):
             order = train_idx.copy()
             np.random.shuffle(order)
+            flags = mirror_flags(self.augment, len(order))
             losses = []
             for a, b in make_batches(len(order), batch_size):
-                planes, policy, value = data.batch(env, order[a:b])
+                planes, policy, value = data.batch(env, order[a:b], mirror=None if flags is None else flags[a:b])
                 losses.append(self.trainer.step(planes, policy, value, lr))
             rec = {"epoch": epoch, "lr": lr, "loss": float(np.mean([l[0] for l in losses])) if losses else None}
             if val is not None:

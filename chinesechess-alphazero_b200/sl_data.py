@@ -236,27 +236,36 @@ class SlDataset:
                          torch.cat([self.values, other.values]),
                          None if self.ply is None else torch.cat([self.ply, other.ply]), visits)
 
-    def batch(self, env, idx, history=False):
+    def batch(self, env, idx, history=False, mirror=None):
         """Training tensors of samples idx (host int array): boards gathered on the device, planes by
         cz_env_encode_planes, the one-hot policy scattered into a zeroed [B][2086] tensor.  history=True: 28 planes,
         planes 14-27 of a sample those of row idx - 2 (the same game's position two plies earlier) where its ply is >= 2,
-        zero otherwise (an empty board encodes to zero planes) — records.expanding_data(..., use_history=True)."""
+        zero otherwise (an empty board encodes to zero planes) — records.expanding_data(..., use_history=True).
+        mirror: optional host array of per-sample flags; a flagged sample is reflected across the central file (its
+        board and history board by cz_env_mirror, its policy target's columns permuted by env.mirror_labels), its value
+        kept."""
         ids = torch.from_numpy(np.ascontiguousarray(idx, np.int64)).to(self.boards.device)
+        flags = None if mirror is None else torch.from_numpy(np.ascontiguousarray(mirror, np.uint8)).to(self.boards.device)
         boards = self.boards.index_select(0, ids)
         if history:
             if self.ply is None:
                 raise ValueError("28-plane batches need the dataset's ply column")
             earlier = self.boards.index_select(0, (ids - 2).clamp_min(0))
             earlier = torch.where((self.ply.index_select(0, ids) >= 2).unsqueeze(1), earlier, torch.zeros_like(earlier))
-            both = env.planes_batch(torch.cat([boards, earlier]))
+            both = torch.cat([boards, earlier])
+            if flags is not None:
+                both = env.mirror(both, torch.cat([flags, flags]))
+            both = env.planes_batch(both)
             planes = torch.cat([both[:len(ids)], both[len(ids):]], dim=1)
         else:
-            planes = env.planes_batch(boards.contiguous())
+            planes = env.planes_batch(boards.contiguous() if flags is None else env.mirror(boards, flags))
         if self.visits is not None:
             policy = self.visit_targets(env.lib, ids)
         else:
             policy = torch.zeros((len(ids), N_LABELS), dtype=torch.float32, device=self.boards.device)
             policy.scatter_(1, self.labels.index_select(0, ids).long().unsqueeze(1), 1.0)
+        if flags is not None:
+            policy = env.mirror_policy(policy, flags)
         return planes, policy, self.values.index_select(0, ids)
 
     def visit_targets(self, lib, ids):

@@ -17,15 +17,15 @@ from . import sl
 logger = getLogger(__name__)
 
 
-def start(config, skip):
-    return SupervisedWorker(config).start(skip)
+def start(config, skip, augment=None):
+    return SupervisedWorker(config, augment=augment).start(skip)
 
 
 class SupervisedWorker(sl.SupervisedWorker):
     LR = 0.003                                     # sl_onegreen.py:82 Adam(lr=0.003)
 
-    def __init__(self, config, trainer_factory=None, device=None, lib=None):
-        super().__init__(config, trainer_factory, device, lib)
+    def __init__(self, config, trainer_factory=None, device=None, lib=None, augment=None):
+        super().__init__(config, trainer_factory, device, lib, augment)
         self.games = None
 
     def start(self, skip=0):

@@ -91,8 +91,9 @@ class Position:
 
 class UCI:
     def __init__(self, config, model=None, lib=None, device=None, stdin=None, stdout=None, use_pipes=False, pipes_factory=None,
-                 infinite_capacity=200000):
+                 infinite_capacity=200000, eval_mirror=False):
         self.config = config
+        self.eval_mirror = eval_mirror          # the player's network averages every leaf and its left-right mirror
         self.lib = lib or get_lib()
         self.device = device
         self.env = StaticEnv(self.lib, device)
@@ -215,7 +216,7 @@ class UCI:
         self.player = CChessPlayer(self.config, search_tree=None, pipes=pipes, enable_resign=False, debugging=True, uci=True,
                                    use_history=self.use_history, side=self.pos.turns % 2, lib=self.lib, device=self.device,
                                    weights=None if pipes is not None else self.model.torch_weights(),
-                                   infinite_capacity=self.infinite_capacity)
+                                   infinite_capacity=self.infinite_capacity, eval_mirror=self.eval_mirror)
         self.player.info_stream = self.stdout
         self.search_worker = Thread(target=self._think, args=(self.player, limits), daemon=True)
         self.search_worker.start()

@@ -49,6 +49,10 @@ int cz_build_is_cuda(void);
  * (from,to) or -1.  Host-only, no device work.
  * ---------------------------------------------------------------------------------------- */
 int cz_action_labels(char* labels_host, int16_t* lut_host);
+/* Left-right mirror of the action labels (x -> 8 - x on both squares; the rules are symmetric across the central file):
+ * lut_host [2086] int16, lut_host[l] = label of l's reflected move.  An involution whose 90 fixed points are the moves
+ * along file 4.  Built from cz_action_labels.  Host-only, no device work. */
+int cz_mirror_labels(int16_t* lut_host);
 
 /* ------------------------------------------------------------------------------------------
  * Batched rules kernels (one warp per board) — environment/static_env.py
@@ -69,6 +73,10 @@ int cz_env_check_catch(const uint8_t* boards_dev, const uint16_t* moves_dev, int
                        uint8_t* be_catched_dev, uint8_t* has_attack_dev, void* stream);
 /* 128-bit canonical position keys (replaces the state-string dict key, agent/player.py:49). */
 int cz_env_keys(const uint8_t* boards_dev, int n, uint64_t* keys_dev /* [n][2] */, void* stream);
+/* Left-right mirror of boards [n][CZ_BOARD_STRIDE]: square y*9+x -> y*9+(8-x), pad bytes copied.  flags_dev [n] may be
+ * NULL (every row mirrored); otherwise a row is mirrored where its flag is nonzero and copied unchanged where it is 0.
+ * boards_dev == out_dev is allowed.  Pairs with cz_mirror_labels: movegen(mirror(b)) = cz_mirror_labels(movegen(b)). */
+int cz_env_mirror(const uint8_t* boards_dev, const uint8_t* flags_dev, int n, uint8_t* out_dev, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Human game records — worker/sl.py load_game :124-174 and worker/sl_onegreen.py load_game :134-175, one warp per game
@@ -162,6 +170,14 @@ typedef struct cz_config {
   int32_t record_visits;       /* 1: the on-device game loop records every ply's root visit counts, calc_policy's N(s,a) with the
                                 * no_act moves zeroed (agent/player.py:375-406; worker/self_play.py:112,134 keep the policy the
                                 * reference commented out).  Read them with cz_drain_records_visits.  Not with arena */
+  int32_t eval_mirror;         /* 1: every evaluation by the engine's own network in the device-driven loop (cz_search,
+                                * cz_search_run, cz_play_move / cz_selfplay, the arena with each range's network) averages the
+                                * leaf b and its left-right mirror Mb (cz_env_mirror):  p(l) = 0.5 * (pi(b)[l] + pi(Mb)[M l]),
+                                * v = 0.5 * (v(b) + v(Mb)), M = cz_mirror_labels, each sum and product rounded once in fp32.  History
+                                * engines mirror both boards of the leaf record.  Costs a second tower pass per leaf: the network's
+                                * batch is 2 * n_games * leaves_per_round.  The host-driven calls (cz_search_wave, cz_leaf_*,
+                                * cz_search_apply*) and cz_nn_forward* are unchanged: they apply what the caller hands them.
+                                * Rejected without a network of the engine's own (nn_filters == 0) */
 } cz_config;
 
 /* Device workspace the caller must provide (a torch.uint8 CUDA tensor). */
