@@ -38,6 +38,24 @@ FIRST_OUT, FIRST_OUT32, LAST_CONV1, TOWER_OUT, TOWER_OUT32, POL_FEAT, LOGITS, ST
 KPOLN = 2304                                  # logits row: 2086 labels padded to 9 tiles of 256
 
 
+def use_n_split(n, c, sms):
+    """cz_nn.cu use_n_split: the residual convs run as 64-column tiles when the M tiles x C / 64 fit one wave of CTAs."""
+    return c > 64 and (n * 90 + 127) // 128 * (c // 64) <= sms
+
+
+def conv_tile_n(c, split=False):
+    """cz_nn.cu conv_tile_n: the conv's N tile."""
+    return 64 if split else 128 if c == 256 else c
+
+
+def conv_tile_m(n, c, sms):
+    """cz_nn.cu conv_tile_m of the full-width conv (and of the trainer's convs, which never split): 256-pixel M tiles once
+    they fill 8 waves of CTAs, else 128; C = 192 and the 64-column small-batch form stay at 128."""
+    if use_n_split(n, c, sms) or c == 192:
+        return 128
+    return 256 if (n * 90 + 255) // 256 * (c // conv_tile_n(c)) >= 8 * sms else 128
+
+
 def _f64(x):
     if isinstance(x, np.ndarray):
         x = torch.from_numpy(x)
@@ -192,6 +210,34 @@ class Mutation:
         return self.fn(got.clone(), ref)
 
 
+class SwapTileRows:
+    """Inside one 256-pixel M tile, pixel rows [a, a + 64) and [b, b + 64) trade places: a = 0, b = 64 is a consumer
+    warpgroup storing its two m64 blocks in swapped order; a = 64, b = 128 is a store row of cw * 64 instead of
+    cw * MB * 64.  The tile is the full one whose two blocks differ most in the reference.  Outputs with one pixel per row
+    and channels last: [n][90][C] or [n * 90][C]."""
+
+    def __init__(self, a, b):
+        self.a, self.b = a, b
+        self.name = f"swap pixel rows {a}..{a + 63} and {b}..{b + 63} of a 256-pixel tile"
+
+    def __call__(self, got, ref):
+        c = got.shape[-1]
+        rows = got.reshape(-1, c)
+        tiles = rows.shape[0] // 256
+        assert tiles >= 1, "no full 256-pixel tile"
+        r = ref.reshape(-1, c)[:tiles * 256].reshape(tiles, 256, c)
+        d = (r[:, self.a:self.a + 64] - r[:, self.b:self.b + 64]).abs().amax(dim=(1, 2))
+        a, b = 256 * int(d.argmax()) + self.a, 256 * int(d.argmax()) + self.b
+        g = rows.clone()
+        g[a:a + 64], g[b:b + 64] = rows[b:b + 64], rows[a:a + 64]
+        return g.reshape(got.shape)
+
+
+def tile256_mutations():
+    """The row placements a 256-pixel tile (two m64 blocks per consumer warpgroup) can get wrong."""
+    return [SwapTileRows(0, 64), SwapTileRows(64, 128)]
+
+
 def assert_rejects(check, got, ref, mutations):
     """`check(got, ref)` raises AssertionError on every mutated copy of `got`; returns the mutation names."""
     got, ref = _f64(got), _f64(ref)
@@ -303,6 +349,26 @@ def positions(n, in_planes=14, seed=0):
     states = [h[-1] if h else osenv.INIT_STATE for h in hists]
     planes = np.stack([osenv.state_history_to_planes(s, h) for s, h in zip(states, hists)])
     return states, planes, [h[-5] if h and len(h) >= 5 else None for h in hists]
+
+
+def distinct_states(n, seed):
+    """n distinct positions, the initial one first, that are not over: every ply of seeded random playouts of up to 120
+    plies.  One oracle step per position (positions() replays a whole playout per position), so thousands take seconds."""
+    rng = np.random.RandomState(seed)
+    out, seen = [osenv.INIT_STATE], {osenv.INIT_STATE}
+    while len(out) < n:
+        s = osenv.INIT_STATE
+        for _ in range(120):
+            lm = osenv.get_legal_moves(s)
+            s = osenv.step(s, lm[rng.randint(len(lm))])
+            if osenv.done(s)[0]:
+                break
+            if s not in seen:
+                seen.add(s)
+                out.append(s)
+                if len(out) == n:
+                    break
+    return out[:n]
 
 
 def boards(cuda_env, states, history, in_planes):

@@ -37,8 +37,11 @@ def test_epilogue_rows_and_offsets(cuda_lib, cuda_env, filters, blocks, n, extra
     n_max = n + extra
     s32 = blocks >= 10                                           # the engine's default skip stream precision
     w = om.init_weights(filters, blocks, 256, seed=filters + blocks, trained_like=True, spread=0.1)
-    states = [osenv.INIT_STATE] + midgame_states(n - 1, 21, lo=1, hi=120)
-    filler = midgame_states(n_max, 22, lo=1, hi=120)
+    if n > 1024:                            # thousands of distinct positions: one oracle step each
+        states, filler = nc.distinct_states(n, 21), nc.distinct_states(n_max, 22)
+    else:
+        states = [osenv.INIT_STATE] + midgame_states(n - 1, 21, lo=1, hi=120)
+        filler = midgame_states(n_max, 22, lo=1, hi=120)
     ahead = midgame_states(front, 23, lo=1, hi=120)
     eng = Engine(cuda_lib, "cuda", n_games=n_max, sims_per_move=8, leaves_per_round=1, nn_filters=filters, nn_blocks=blocks,
                  nn_value_fc=256)

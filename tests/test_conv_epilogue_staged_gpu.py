@@ -9,14 +9,17 @@ batch); the cases add
   5 others (a partial last tile, every position in a differently placed tile) must come out bit-identical, which makes the
   offset check an equality between the two epilogues;
 * 377 boards = 265 full tiles and a partial one, more than two tiles per CTA on 132 SMs: the staging ring wraps inside a tile
-  and across tiles while the previous tile's stores are still in flight."""
+  and across tiles while the previous tile's stores are still in flight;
+* 1573 boards at C = 256 and 3109 at C = 128 (and the engine's 1610 and 3146 rows): 256-pixel M tiles, each consumer
+  warpgroup storing two m64 blocks through its ring per tile, and a last tile of 2 pixels."""
 import pytest
 
 from tests.test_conv_epilogue_gpu import test_epilogue_rows_and_offsets as _check
 
 pytestmark = pytest.mark.gpu
 
-CASES = [(256, 20, 64, 37, 5), (128, 7, 64, 37, 5), (256, 20, 377, 37, 5), (128, 7, 377, 37, 5)]
+CASES = [(256, 20, 64, 37, 5), (128, 7, 64, 37, 5), (256, 20, 377, 37, 5), (128, 7, 377, 37, 5),
+         (256, 20, 1573, 37, 5), (128, 7, 3109, 37, 5)]
 
 
 @pytest.mark.parametrize("filters,blocks,n,extra,front", CASES, ids=lambda v: str(v))

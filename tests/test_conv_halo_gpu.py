@@ -1,7 +1,7 @@
 """The 3x3 conv's halo-resident A operand (k_igemm conv mode) at the batch shapes that separate its cases.
 
 An M tile of the full-width conv is 256 pixels when such tiles fill at least 8 waves of CTAs (C = 256 from 1500 boards,
-C = 128 from 3001 on 132 SMs), else 128; its producer loads the tile's input rows plus 10 rows either side once, and every tap
+C = 64 and 128 from 3001 on 132 SMs), else 128; its producer loads the tile's input rows plus 10 rows either side once, and every tap
 reads them at a row offset, with taps that fall off the board pointed at a row of zeros.  Cases:
 
 * pixel counts just below, at and just above a multiple of 256 (90 n is even: n = 91 + 128 k gives 256 j - 2, n = 128 k
@@ -51,7 +51,7 @@ def _inputs(n, c, seed, residual):
 
 
 CASES = ([(c, n) for c in (256, 128, 192) for n in (1, 37, 91, 128)]      # 128-pixel tiles
-         + [(256, n) for n in (1627, 1536, 1573)] + [(128, n) for n in (3035, 3072, 3109)])   # 256-pixel tiles
+         + [(256, n) for n in (1627, 1536, 1573)] + [(c, n) for c in (128, 64) for n in (3035, 3072, 3109)])   # 256-pixel tiles
 
 
 @pytest.mark.parametrize("c,n", CASES, ids=lambda v: str(v))

@@ -109,3 +109,34 @@ def test_bound_arithmetic():
 
 def test_read_buffer_is_unsupported_in_the_emulation_build(emul_lib):
     assert emul_lib.raw("cz_nn_read_buffer")(None, nc.LOGITS, 1, None, 0, None) == -5     # CZ_ERR_UNSUPPORTED
+
+
+def test_conv_tile_restatement():
+    """256-pixel M tiles from 1500 boards at C = 256 and from 3001 at C = 64 and 128 on 132 SMs; never at C = 192 or in
+    the 64-column small-batch form."""
+    for c, first in ((256, 1500), (128, 3001), (64, 3001)):
+        assert nc.conv_tile_m(first - 1, c, 132) == 128 and nc.conv_tile_m(first, c, 132) == 256, c
+    assert nc.conv_tile_m(20000, 192, 132) == 128
+    assert nc.use_n_split(9, 256, 132) and nc.conv_tile_m(9, 256, 132) == 128
+    assert not nc.use_n_split(20000, 64, 132)
+
+
+def test_distinct_states_are_distinct_and_live():
+    states = nc.distinct_states(500, seed=1)
+    assert len(set(states)) == 500 and states[0] == nc.osenv.INIT_STATE
+    assert not any(nc.osenv.done(s)[0] for s in states)
+    assert states == nc.distinct_states(500, seed=1) and states != nc.distinct_states(500, seed=2)
+
+
+def test_tile_row_swaps_are_rejected_on_the_reference_itself(small_net):
+    """Both 256-pixel tile mutations move rows of a conv output far outside the bound (9 boards = 3 full tiles)."""
+    w, planes, fo, st = small_net
+    first, s0 = nc.first_conv_ref(planes, fo, "cpu")
+    c1, s1 = nc.res_conv_ref(first, fo, 0)
+    check = lambda g, r: nc.check_close(g, r, s1, "fp16")
+    assert nc.assert_rejects(check, c1, c1, nc.tile256_mutations()) == [m.name for m in nc.tile256_mutations()]
+    flat = c1.reshape(-1, c1.shape[-1])
+    bad = nc.SwapTileRows(0, 64)(flat, flat)
+    assert torch.equal(bad.reshape(c1.shape), nc.SwapTileRows(0, 64)(c1, c1))
+    moved = (bad != flat).any(dim=1).nonzero().flatten().tolist()       # rows 0..127 of one tile, nothing else
+    assert moved and moved[0] % 256 == 0 and set(moved) <= set(range(moved[0], moved[0] + 128))

@@ -10,7 +10,9 @@ would have failed on a subtly wrong kernel.
 The cases cover the branches of the kernels: C = 64 (no N-split) .. 256; n = 1 (one partial M tile), 9 (64-column
 N-split tiles, one position per k_heads block), 64 and 301 (full-width tiles, partial last M tile, 4 positions per
 k_heads block with one position in the last block); fp32 skip stream on and off; head widths (4, 2), (2, 4) and (32, 4)
-(K = 8640 in the policy GEMM, > 48 KB of shared memory in k_heads); 14 and 28 input planes."""
+(K = 8640 in the policy GEMM, > 48 KB of shared memory in k_heads); 14 and 28 input planes; and 1536 to 3109 distinct
+positions, where the residual convs run 256-pixel M tiles with full, nearly empty and nearly full last tiles.  Together
+the cases reach every conv kernel instance launch_igemm can choose and every epilogue form of each."""
 import ctypes as C
 
 import numpy as np
@@ -18,6 +20,7 @@ import pytest
 import torch
 
 from oracle import model as om
+from oracle import senv as osenv
 from tests import nn_checks as nc
 
 pytestmark = pytest.mark.gpu
@@ -34,6 +37,14 @@ ONE_BLOCK = [
     (256, 1, 9, True, 4, 2, 28),
     (256, 1, 64, False, 32, 4, 14),
     (256, 1, 301, False, 4, 2, 14),
+    # 256-pixel M tiles (two m64 blocks per consumer warpgroup) on 132 SMs; the last tile holds 90 n mod 256 pixels
+    (256, 1, 1573, True, 4, 2, 14),        # 2
+    (256, 1, 1536, False, 4, 2, 14),       # 0: no partial tile
+    (256, 1, 1627, True, 2, 4, 14),        # 254
+    (128, 1, 3109, False, 4, 2, 14),       # 2
+    (128, 1, 3072, True, 4, 2, 14),        # 0
+    (64, 1, 3035, False, 4, 2, 14),        # 254
+    (64, 1, 3109, True, 4, 2, 14),         # 2
 ]
 DEEP = [(192, 10, 64, None, 4, 2, 14), (256, 20, 64, None, 4, 2, 14)]
 ALL = ONE_BLOCK + DEEP
@@ -49,11 +60,6 @@ def _id(case):
     return f"{c}x{b}-n{n}-{'auto' if s32 is None else ('f32' if s32 else 'f16')}skip-h{pc}.{vc}-p{planes}"
 
 
-def use_n_split(n, c, sms):
-    """cz_nn.cu use_n_split: the residual convs run as 64-column tiles when the M tiles x C / 64 fit one wave of CTAs."""
-    return c > 64 and (n * 90 + 127) // 128 * (c // 64) <= sms
-
-
 class Run:
     """One forward of a case on the GPU with every buffer read back, its operands and its float64 reference."""
 
@@ -62,7 +68,11 @@ class Run:
         c, blocks, n, s32, pc, vc, in_planes = case
         self.c, self.blocks, self.n, self.pc = c, blocks, n, pc
         self.s32 = blocks >= 10 if s32 is None else s32
-        states, planes, hist = nc.positions(n, in_planes, seed=c + n)
+        if n > 1024:                                       # one ply per position: thousands of distinct positions in seconds
+            states = nc.distinct_states(n, seed=c + n)
+            planes, hist = np.stack([osenv.state_to_planes(s) for s in states]), [None] * n
+        else:
+            states, planes, hist = nc.positions(n, in_planes, seed=c + n)
         self.planes = torch.from_numpy(planes).cuda()
         self.w = nc.well_conditioned_weights(c, blocks, planes, seed=c + blocks + pc, device="cuda", in_planes=in_planes,
                                              policy_filters=pc, value_filters=vc)
@@ -100,29 +110,69 @@ class Run:
         return (hi.double() + lo.double())[:, :self.pc * 90]
 
 
-_runs = {}                                                 # every stage test of a case checks the same forward
+# Every stage test of a case checks the same forward.  A run of more than 1024 positions holds float64 stage tensors of
+# a few hundred MB each, so at most one of those is kept: the parametrizations are module-scoped, which makes pytest run
+# all the tests of one case back to back.
+_runs = {}
+BIG = 1024
 
 
 def _run(case, cuda_lib, cuda_env):
     if case not in _runs:
+        if case[2] > BIG:
+            for k in [k for k in _runs if k[2] > BIG]:
+                del _runs[k]
+            torch.cuda.empty_cache()
         _runs[case] = Run(case, cuda_lib, cuda_env)
     return _runs[case]
+
+
+def _sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def _conv_mutations(r):
+    """The 256-pixel tiles' own row placements on top of the checks every case runs."""
+    return nc.tile256_mutations() if nc.conv_tile_m(r.n, r.c, _sms()) == 256 else []
 
 
 def _report(stage, case, value):
     print(f"\n[nn-stage] {stage:<14} {_id(case):<36} {value:.3g}")
 
 
+def conv_forms(case, sms):
+    """(kernel instance N_TILE x M_TILE, epilogue form) of the residual convs of a 1-block case, restated from cz_nn.cu and
+    k_igemm: conv1 (no skip) leaves its full M tiles by the staged epilogue and a partial last tile from registers; conv2
+    adds the skip stream in registers, fp16 or fp32 (then also writing the fp32 copy out32)."""
+    c, _, n, s32, *_ = case
+    tm = nc.conv_tile_m(n, c, sms)
+    inst = f"{nc.conv_tile_n(c, nc.use_n_split(n, c, sms))}x{tm}"
+    forms = {"fp32 skip + out32" if s32 else "fp16 skip"}
+    if n * 90 >= tm:
+        forms.add("staged")
+    if n * 90 % tm:
+        forms.add("register, no skip")
+    return {(inst, f) for f in forms}
+
+
 def test_cases_cover_both_conv_paths(cuda_lib):
-    """The residual convs take the N-split small-batch path or the full-width one depending on the SM count; the cases above
-    run both for C = 128 and C = 256 on this device."""
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    """The residual convs take the N-split small-batch path or the full-width one depending on the SM count, and 128- or
+    256-pixel M tiles; the 1-block cases above run both paths for C = 128 and C = 256 on this device, and every conv kernel
+    instance launch_igemm can choose with every epilogue form."""
+    sms = _sms()
     for c in (128, 256):
-        assert {use_n_split(n, c, sms) for (cc, _, n, *_rest) in ALL if cc == c} == {True, False}, (c, sms)
-    assert any(use_n_split(n, c, sms) for (c, _, n, *_r) in ONE_BLOCK) and any(n > 2 * sms for (_, _, n, *_r) in ALL)
+        assert {nc.use_n_split(n, c, sms) for (cc, _, n, *_rest) in ALL if cc == c} == {True, False}, (c, sms)
+    assert any(nc.use_n_split(n, c, sms) for (c, _, n, *_r) in ONE_BLOCK) and any(n > 2 * sms for (_, _, n, *_r) in ALL)
+    reached = set().union(*(conv_forms(case, sms) for case in ONE_BLOCK))
+    for inst, form in sorted(reached):
+        print(f"\n[nn-stage] reached {inst:<8} {form}")
+    instances = {"64x128", "64x256", "128x128", "128x256", "192x128"}
+    forms = {"staged", "register, no skip", "fp16 skip", "fp32 skip + out32"}
+    assert {(i, f) for i in instances for f in forms} <= reached, sorted({(i, f) for i in instances for f in forms} - reached)
+    assert {i for i, _ in reached} == instances
 
 
-@pytest.mark.parametrize("case", ONE_BLOCK, ids=_id)
+@pytest.mark.parametrize("case", ONE_BLOCK, ids=_id, scope="module")
 def test_first_conv(cuda_lib, cuda_env, case):
     """k_conv_first: 5x5 conv of the one-hot planes (gathered from packed boards) + BN + ReLU, fp32 sums, fp16 out."""
     r = _run(case, cuda_lib, cuda_env)
@@ -135,17 +185,17 @@ def test_first_conv(cuda_lib, cuda_env, case):
         assert torch.equal(r.first, r.first32.half())      # fp16 output = RN(fp32 output), bit for bit
 
 
-@pytest.mark.parametrize("case", ONE_BLOCK, ids=_id)
+@pytest.mark.parametrize("case", ONE_BLOCK, ids=_id, scope="module")
 def test_conv1(cuda_lib, cuda_env, case):
     """k_igemm conv1 of the block (BN + ReLU) on the GPU's first-conv output."""
     r = _run(case, cuda_lib, cuda_env)
     ref, s = nc.res_conv_ref(r.first, r.fo, 0)
     check = lambda g, rf: nc.check_close(g, rf, s, "fp16", what="LAST_CONV1")
     _report("conv1", case, check(r.conv1, ref))
-    nc.assert_rejects(check, r.conv1, ref, [nc.AddTerm(s, 9 * r.c), nc.ShiftBlock()])
+    nc.assert_rejects(check, r.conv1, ref, [nc.AddTerm(s, 9 * r.c), nc.ShiftBlock()] + _conv_mutations(r))
 
 
-@pytest.mark.parametrize("case", ONE_BLOCK, ids=_id)
+@pytest.mark.parametrize("case", ONE_BLOCK, ids=_id, scope="module")
 def test_conv2_with_skip(cuda_lib, cuda_env, case):
     """k_igemm conv2 (BN, + skip from the first conv in fp16 or fp32, ReLU; fp32 copy for the next block) on the GPU's conv1."""
     r = _run(case, cuda_lib, cuda_env)
@@ -153,13 +203,13 @@ def test_conv2_with_skip(cuda_lib, cuda_env, case):
     ref, s = nc.res_conv_ref(r.conv1, r.fo, 1, skip)
     check = lambda g, rf: nc.check_close(g, rf, s, "fp16", what="TOWER_OUT")
     _report("conv2", case, check(r.tower, ref))
-    nc.assert_rejects(check, r.tower, ref, [nc.AddTerm(s, 9 * r.c), nc.ShiftBlock(), nc.DropResidual(skip)])
+    nc.assert_rejects(check, r.tower, ref, [nc.AddTerm(s, 9 * r.c), nc.ShiftBlock(), nc.DropResidual(skip)] + _conv_mutations(r))
     if r.s32:
         _report("conv2_32", case, nc.check_close(r.tower32, ref, s, "fp32", what="TOWER_OUT32"))
         assert torch.equal(r.tower, r.tower32.half())
 
 
-@pytest.mark.parametrize("case", DEEP, ids=_id)
+@pytest.mark.parametrize("case", DEEP, ids=_id, scope="module")
 def test_deep_tower_end_to_end(cuda_lib, cuda_env, case):
     """The whole residual tower of a deep net from the boards: relative Frobenius error against the float64 tower."""
     r = _run(case, cuda_lib, cuda_env)
@@ -171,7 +221,7 @@ def test_deep_tower_end_to_end(cuda_lib, cuda_env, case):
     assert e < DEEP_TOWER_REL[r.blocks], e
 
 
-@pytest.mark.parametrize("case", ALL, ids=_id)
+@pytest.mark.parametrize("case", ALL, ids=_id, scope="module")
 def test_heads_policy_features(cuda_lib, cuda_env, case):
     """k_heads: 1x1 policy conv + BN + ReLU in fp32, Keras Flatten (c * 90 + pix), split into fp16 [hi | lo | hi]."""
     r = _run(case, cuda_lib, cuda_env)
@@ -187,7 +237,7 @@ def test_heads_policy_features(cuda_lib, cuda_env, case):
     nc.assert_rejects(check, got, r.feat_ref, [nc.AddTerm(r.feat_scale, r.c, "hilo"), nc.ShiftBlock()])
 
 
-@pytest.mark.parametrize("case", ALL, ids=_id)
+@pytest.mark.parametrize("case", ALL, ids=_id, scope="module")
 def test_heads_value(cuda_lib, cuda_env, case):
     """k_heads value MLP (1x1 conv + BN + ReLU, Dense + ReLU, Dense, tanh), compared before tanh as atanh(value); tanhf's
     two ulps are stretched by 1 / (1 - v^2) there."""
@@ -200,7 +250,7 @@ def test_heads_value(cuda_lib, cuda_env, case):
     nc.assert_rejects(check, got, r.vpre_ref, [nc.AddTerm(r.vpre_scale, 256, "fp32")])
 
 
-@pytest.mark.parametrize("case", ALL, ids=_id)
+@pytest.mark.parametrize("case", ALL, ids=_id, scope="module")
 def test_policy_gemm_split_precision(cuda_lib, cuda_env, case):
     """The policy Dense on wgmma as one split-precision GEMM ([x_hi | x_lo | x_hi] . [w_hi | w_hi | w_lo]) against the
     float64 product with the UNSPLIT fp32 kernel: within BETA * S with no extra slack, i.e. fp32 accuracy."""
@@ -225,7 +275,7 @@ def _check_stats(stats, logits):
     return worst
 
 
-@pytest.mark.parametrize("case", ALL, ids=_id)
+@pytest.mark.parametrize("case", ALL, ids=_id, scope="module")
 def test_gemm_row_stats(cuda_lib, cuda_env, case):
     r = _run(case, cuda_lib, cuda_env)
     logits = r.logits[:, :nc.N_LABELS]
@@ -244,7 +294,7 @@ def test_gemm_row_stats(cuda_lib, cuda_env, case):
                                                nc.Mutation("last tile's max one ulp low", last_max)])
 
 
-@pytest.mark.parametrize("case", ALL, ids=_id)
+@pytest.mark.parametrize("case", ALL, ids=_id, scope="module")
 def test_softmax(cuda_lib, cuda_env, case):
     """k_softmax (finishing the epilogue's statistics) against the float64 softmax of the GPU's logits."""
     r = _run(case, cuda_lib, cuda_env)

@@ -82,7 +82,8 @@ def test_wgrad_matches_float64(cuda_lib, c, n):
     print(f"wgrad C={c} n={n}: worst err/bound {worst:.3g}")
 
 
-DGRAD_CASES = [(64, 7), (128, 256), (192, 1), (256, 1024)]
+# the last three run the fp32-output conv on 256-pixel M tiles (two m64 blocks per consumer warpgroup) on 132 SMs
+DGRAD_CASES = [(64, 7), (128, 256), (192, 1), (256, 1024), (256, 1573), (128, 3109), (64, 3035)]
 
 
 @pytest.mark.parametrize("c,n", DGRAD_CASES)
@@ -103,7 +104,10 @@ def test_dgrad_matches_float64(cuda_lib, c, n):
         return nc.check_close(got, r, flat(s), out="fp32", what=f"dgrad C={c} n={n}")
 
     worst = check(dx, flat(ref))
-    nc.assert_rejects(check, dx, flat(ref), [nc.Mutation("dgrad without the tap flip", lambda g_, r: flat(noflip).clone())])
+    muts = [nc.Mutation("dgrad without the tap flip", lambda g_, r: flat(noflip).clone())]
+    if nc.conv_tile_m(n, c, torch.cuda.get_device_properties(0).multi_processor_count) == 256:
+        muts += nc.tile256_mutations()
+    nc.assert_rejects(check, dx, flat(ref), muts)
     print(f"dgrad C={c} n={n}: worst err/bound {worst:.3g}")
 
 

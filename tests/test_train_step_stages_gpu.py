@@ -273,14 +273,20 @@ CASES = [
     ("1blk-c64-b7", 64, 1, 14, (4, 2, 256), 7, 2.0, {"dFp_split"}),
     ("1blk-c192-b256", 192, 1, 14, (4, 2, 256), 256, 2.0, {"dWp_split"}),
     ("10blk-c192-b1024", 192, 10, 14, (4, 2, 256), 1024, 2.0, {"bn_cap", "dWp_split"}),
+    # 256-pixel conv tiles.  P = 1024 x 270 fills the last BN column chunk: a dropped last chunk then moves a batch
+    # variance by 1/1024 of it, as at 10blk-c192-b1024, under the smaller conv bound of C = 128.  (At 1573 x 256 the last of
+    # 1019 chunks holds 68 rows, and dropping it stays within the conv's propagated bound.)
+    ("1blk-c128-b3072", 128, 1, 14, (4, 2, 256), 3072, 2.0, {"conv_m256", "bn_cap", "dWp_split"}),
 ]
 
 
-def geometry_paths(n, C_, heads):
+def geometry_paths(n, C_, heads, blocks):
     """Which launch paths the restated geometry predicts for this shape."""
     pc, vc, H = heads
     pk, vk, P = pc * 90, vc * 90, n * 90
     paths = set()
+    if blocks and nc.conv_tile_m(n, C_, torch.cuda.get_device_properties(0).multi_processor_count) == 256:
+        paths.add("conv_m256")                      # the residual block's convs and dgrads on 256-pixel M tiles
     ch, per = first_wgrad_geometry(n)
     if ch == 2:
         paths.add("fw_chunks2")
@@ -306,12 +312,12 @@ def geometry_paths(n, C_, heads):
 def test_geometry_restatement_reaches_every_path():
     """The cases below reach every split / chunk path of the step's launch code (host-only arithmetic)."""
     hit = set()
-    for _, c, _, _, heads, n, _, want in CASES:
-        got = geometry_paths(n, c, heads)
+    for _, c, blocks, _, heads, n, _, want in CASES:
+        got = geometry_paths(n, c, heads, blocks)
         assert want <= got, (n, c, heads, want - got)
         hit |= got
-    assert {"fw_chunks2", "fw_partial", "fw_256", "bn_cap", "logits_split", "dFp_split", "value_split", "dbd_split",
-            "dWp_split"} <= hit
+    assert {"conv_m256", "fw_chunks2", "fw_partial", "fw_256", "bn_cap", "logits_split", "dFp_split", "value_split",
+            "dbd_split", "dWp_split"} <= hit
     assert first_wgrad_geometry(1000) == (16, 63) and 1000 - 15 * 63 == 55
     assert first_wgrad_geometry(4096) == (16, 256)
     assert col_chunks(729 * 90)[0] <= 1024 < -(-729 * 90 // 64)
@@ -324,7 +330,7 @@ def test_train_step_stages_match_float64(cuda_lib, case):
     cid, C_, L, ip, heads, n, logit_std, want = case
     pc, vc, H = heads
     pk, vk, P = pc * 90, vc * 90, n * 90
-    assert want <= geometry_paths(n, C_, heads)
+    assert want <= geometry_paths(n, C_, heads, L)
     dev = "cuda"
     seed = n + 7 * L + C_
     planes = positions(n, ip, seed % 5)
@@ -680,7 +686,7 @@ def test_train_step_stages_match_float64(cuda_lib, case):
             return nc.check_close(g, r, Sy1 * (beta(7) / nc.BETA), out="fp16", extra=ey1, what=f"{cid}: res{L} conv1 output (fp16)")
         R.rows.append((f"res{L} conv1 + BN + ReLU (h16)", chk_h16(f64(h16), torch.relu(y1)), 1))
         nc.assert_rejects(lambda g, r: chk_h16(g.reshape(P, C_), r), f64(h16).reshape(n, 90, C_), torch.relu(y1),
-                          [nc.ShiftBlock(64)])
+                          [nc.ShiftBlock(64)] + (nc.tile256_mutations() if "conv_m256" in want else []))
         y2, Sy2, ey2 = bn_apply(z2, zb2, m2, var2, W(f"res{L}_batchnorm2", "gamma"), W(f"res{L}_batchnorm2", "beta"), s_prev)
         R.check(f"res{L} output (s32[{L}])", SL, torch.relu(y2), Sy2, 7, ey2,
                 [nc.Mutation("residual dropped from one channel",
